@@ -13,13 +13,13 @@ output records, issued on a side stream so that it overlaps the next step's trun
 `e2e`    : same metric through the public host-buffer API (mnc_b200.api.Detector.im_detect_images):
            uint8 frames in host memory -> H2D -> prep + forward -> results D2H, all inside the
            timed region; reported from page-locked and from pageable caller memory.
-`roofline`: the dominant kernel (tcgen05 implicit GEMM: all conv + inner-product launches of a step):
+`roofline`: the dominant kernel (wgmma implicit GEMM: all conv + inner-product launches of a step):
            algorithmic FLOPs (2*M*N*K, real dims) / summed per-launch CUDA-event time (measured in
            an eager pass of the same step); `roofline_roi_warp`: the RoI-warp HBM roofline.
 `micro`  : BASELINE.json configs[3] (RoI-warp / mask-pool GB/s) and configs[4] (gpu_nms 10k boxes,
            gpu_mask_voting 600 x 21; ms + bit-exactness against the reference's own kernels).
 `cpu_baseline`: the oracle (port of the reference path; the reference has no runnable CPU path,
-           BASELINE.md section 2) timed on this box's host cores on a bounded sample (rank 0, N=1).
+           BASELINE.md section 2) timed on the host cores on a bounded sample (rank 0, N=1).
 --impl reference prints the same line for the CPU oracle alone.
 """
 import argparse
@@ -38,12 +38,20 @@ METRIC = "images/sec VGG16 MNC 5-stage @600x1000, 300 RoIs"
 
 
 def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    """Data-sheet figures of the H100 SXM at its 700 W limit (dense BF16 / FP16, HBM3): ceilings for
+    the roofline fractions, not measured rates -- a card with a lower power limit sustains less."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "NVIDIA H100 SXM data sheet"
+
+
+def gpu_identity(index=0):
+    """Name and power limit of the card the numbers were taken on (they are part of the numbers)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        name, limit = [x.strip() for x in out.stdout.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit_w": float(limit)}
+    except Exception:
+        return {"name": None, "power_limit_w": None}
 
 
 def physical_cores():
@@ -69,7 +77,7 @@ def physical_cores():
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -234,10 +242,31 @@ def run_reference(args, rank):
                          "per_image_s": st},
         "e2e": {"value": v, "unit": "images/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "note": "reference has no runnable CPU path (BASELINE.md section 2); oracle port timed on "
-                "%d host threads = usable cores of this container (torch CPU fp32 conv/FC + numpy layers + C/OpenMP kernels); "
+                "%d host threads = usable cores (torch CPU fp32 conv/FC + numpy layers + C/OpenMP kernels); "
                 "steps/warmup clamped to keep the run bounded" % ncpu,
     }
     _emit(line)
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, tensors):
+    """Write each tensor as out_dir/<name>.npy in float32 (flags such as `valid` become 0.0 / 1.0),
+    at most DUMP_LIMIT_BYTES in all: a tensor over its share of the limit is stored as a fixed,
+    seeded sample of its flattened elements (the sorted indices go to <name>.idx.npy as float64), so
+    that two builds run with the same arguments write comparable files."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: t.detach().float().cpu().numpy() for k, t in tensors.items()}
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, a in arrays.items():
+        if a.nbytes > share:
+            keep = share // 12          # 4 B per value + 8 B per index
+            idx = np.sort(np.random.default_rng(1234).choice(a.size, size=keep, replace=False))
+            np.save(os.path.join(out_dir, name + ".idx.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def workload_config(args, world):
@@ -247,7 +276,7 @@ def workload_config(args, world):
             "parallelism": "dp%d (images sharded, 1 all-gather of records per step, overlapped)" % world,
             "steps_in_flight": 1 if args.no_graph else args.streams,
             "l2": "inputs larger than L2: every step streams 1.13 GB of weights and > 5 GB of "
-                  "activations through the 126 MB L2, nothing of a step survives to the next",
+                  "activations through the 50 MB L2, nothing of a step survives to the next",
             "weights": "seeded random init (mnc_b200/weights.py), fp32 -> fp16 + 2 x e4m3 planes "
                        "(every conv3x3 / inner product; conv1_1, K = 27: split bf16)"}
 
@@ -358,13 +387,9 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="eager launches instead of CUDA-graph replay")
     ap.add_argument("--no-overlap-heads", action="store_true",
                     help="A/B: issue the box branch in line instead of on the side stream")
-    ap.add_argument("--halo-split", action="store_true",
-                    help="A/B: the halo kernel (Cout <= 128 convs) on split-bf16 operands")
     ap.add_argument("--streams", type=int, default=2, choices=[1, 2],
                     help="steps in flight: 2 = consecutive steps alternate between two streams (each "
                          "with its own activation buffers and CUDA graph over the shared weights)")
-    ap.add_argument("--halo-single", action="store_true",
-                    help="A/B: the halo kernel with one CTA per tile instead of CTA pairs")
     ap.add_argument("--nms-matrix", action="store_true",
                     help="A/B: proposal NMS through the n x n/64 suppression matrix (nms_mask + nms_scan) "
                          "instead of the capped form")
@@ -377,8 +402,14 @@ def main():
                     help="A/B: mask voting finds the tight boxes by one full sweep instead of two passes")
     ap.add_argument("--dump-igemm", default=None,
                     help="write the ordered list of tensor-core launches of one step "
-                         "(shape, algorithmic FLOPs / bytes) as JSON, for scripts/ncu_tc_summary.py")
+                         "(shape, algorithmic FLOPs / bytes) as JSON")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned (boxes, masks, "
+                         "scores, valid) as DIR/<name>.npy in float32, 64 MB at most (larger arrays as "
+                         "a fixed seeded sample)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     _claim_stdout()
     # a run that is still going after 5 minutes leaves the Python stacks of all threads on stderr
     # (the default line takes ~20 s on a warm box; one run of the round stalled without a trace)
@@ -406,11 +437,6 @@ def main():
     dev = torch.device("cuda", local)
     B = args.batch
     w = Wt.make_weights(Wt.FULL_ARCH)
-    if args.halo_split:
-        from mnc_b200 import engine as _eng
-        _eng.MNCEngine.HALO_TRI = False
-    if args.halo_single:
-        dense.set_halo_pair(0)
     if args.nms_matrix:
         ops.nms_set_lazy(0)
     if args.nms_single_cta:
@@ -501,8 +527,9 @@ def main():
     t_wall0 = time.perf_counter()
     ev[0].record()
     fork()
+    last = None
     for k in range(args.steps):
-        step_k(k)
+        last = step_k(k)
         if k + 1 < args.steps:
             ev[k + 1].record(streams[k % n_str] if n_str > 1 else None)
     join()
@@ -512,6 +539,9 @@ def main():
     torch.cuda.nvtx.range_pop()
     t_wall = time.perf_counter() - t_wall0
     dev_ms = ev[0].elapsed_time(ev[args.steps])
+    if args.dump_outputs and rank == 0:
+        # the arrays detect_graphed handed back for the last timed step (its engine has not run since)
+        dump_outputs(args.dump_outputs, dict(zip(("boxes", "masks", "scores", "valid"), last[0][:4])))
     step_ms = sorted(ev[k].elapsed_time(ev[k + 1]) for k in range(args.steps))
     clocks = sampler.finish() if rank == 0 else None
     tms = torch.tensor([dev_ms], dtype=torch.float64, device=dev)
@@ -636,28 +666,17 @@ def main():
     flops_step = sum(m["flops"] for m in man)
     k_ms_step = k_ms / n_eager
     peaks, peak_src = _peaks()
-    peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops")))
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
+    peak_tf = float(peaks["bf16_tflops"])
+    hbm = float(peaks["hbm_gbs"])
     ach = flops_step / (k_ms_step / 1000.0) / 1e12 if k_ms_step > 0 else 0.0
-    traffic, traffic_note = None, None
-    for nm in ("r02_ncu_tc_summary.json", "r01_ncu_tc_summary.json"):
-        summ = os.path.join(ROOT, "profiles", nm)
-        if os.path.exists(summ):
-            with open(summ) as f:
-                sj = json.load(f)
-            traffic = sj["mean_traffic_bytes_per_launch"]
-            traffic_note = ("dram__bytes_read.sum + dram__bytes_write.sum per launch, mean over the %d "
-                            "tensor-core launches of one step in the committed ncu --set full capture "
-                            "(profiles/%s); algorithmic bytes of the same launches: %.3e per launch"
-                            % (sj["n_launches"], nm, sj["mean_algorithmic_bytes_per_launch"]))
-            break
     ms_step = total_ms / args.steps
     roofline = {
-        "kernel": "igemm_tc_kernel / conv_halo_tc_kernel (tcgen05 implicit GEMM: 13 conv3x3 + 15 "
+        "kernel": "igemm_tc_kernel (wgmma implicit GEMM: 13 conv3x3 + 15 "
                   "inner-product launches per step)",
         "bound": "tensor", "achieved": ach, "peak": peak_tf, "unit": "TFLOP/s",
-        "frac": ach / peak_tf, "traffic": traffic, "traffic_note": traffic_note,
-        "peak_source": peak_src + ", bf16 dense sustained (kernel timed inside a long step)",
+        "frac": ach / peak_tf, "traffic": None,
+        "peak_source": peak_src + ", bf16 dense, at the 700 W limit: on a card whose `gpu.power_limit_w` "
+                       "is lower the fractions are against a ceiling it cannot reach",
         "launches_timed": k_n, "share_of_step": k_ms_step / ms_step,
         "ms_by_launch_site": [[t, round(m, 4)] for t, m in zip(site_tags, site_ms)],
         "algorithmic_flops_per_step": flops_step,
@@ -696,9 +715,8 @@ def main():
         "metric": METRIC, "value": value, "unit": "images/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None,
-        "dtype": "f16+2xf8 (fp16 main product + two e4m3 correction products on tcgen05, fp32 "
-                 "accumulate, fp32-parity; conv1_1, K = 27: bf16x3)" if not args.halo_split else
-                 "f16+2xf8 (Cout > 128 convs, inner products), bf16x3 (Cout <= 128 convs)",
+        "dtype": "f16+2xf8 (fp16 main product + two e4m3 correction products on wgmma, fp32 "
+                 "accumulate, fp32-parity; conv1_1, K = 27: bf16x3)",
         "data": "synthetic", "config": workload_config(args, world),
         "e2e": {"value": e2e_pinned, "unit": "images/s", "h2d_bytes_per_step": det.h2d_bytes,
                 "d2h_bytes_per_step": det.d2h_bytes,
@@ -712,7 +730,7 @@ def main():
                        "(value_blocking_calls: one synchronous call per step)"
                        + ("; + all-gather of the records" if world > 1 else "")},
         "gpu_launches": launches_per_step * args.steps, "gpu_launches_per_step": launches_per_step,
-        "clocks": clocks, "roofline": roofline, "roofline_roi_warp": roof_warp, "micro": micro,
+        "gpu": gpu_identity(local), "clocks": clocks, "roofline": roofline, "roofline_roi_warp": roof_warp, "micro": micro,
         "cpu_baseline": cpu,
         "step_ms": {"median": step_ms[len(step_ms) // 2], "p10": step_ms[int(0.1 * len(step_ms))],
                     "p90": step_ms[min(len(step_ms) - 1, int(0.9 * len(step_ms)))]},

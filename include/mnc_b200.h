@@ -1,5 +1,5 @@
 /*
- * mnc_b200 -- C-ABI of the B200-native MNC (Multi-task Network Cascades) inference hot path.
+ * mnc_b200 -- C-ABI of the H100-native (sm_90a) MNC (Multi-task Network Cascades) inference hot path.
  *
  * Every entry point is `extern "C"`, takes plain pointers / sizes / a `cudaStream_t` passed as
  * `void*`, and returns an `int` status (MNC_OK == 0).  No torch types cross this boundary.
@@ -48,7 +48,7 @@ int mnc_device_count(void);
  *               (pooling_layer.cu:11-47, pooling_layer.cpp:90-93)
  *   output element (pixel p, channel c) at p*out_pix_stride + out_ch_offset + c
  *   split_k > 1 (fp32 mode only): partial sums go to plane s at s*split_stride; finish with
- *   mnc_splitk_reduce.  bn: Cout tile (0 = auto, 64/128/256).  max_ctas: 0 = one CTA per SM.
+ *   mnc_splitk_reduce.  bn: widest Cout tile (0 = auto; 64 or 128 columns exist, 192 / 256 run as 128).  max_ctas: 0 = one CTA per SM.
  */
 int mnc_igemm_tc(const void* a_hi, const void* a_lo, int batch, int H, int W, int Cin,
                  const void* w_hi, const void* w_lo, int Cout, int taps, const float* bias,
@@ -62,7 +62,7 @@ int mnc_igemm_tc(const void* a_hi, const void* a_lo, int batch, int H, int W, in
  *   k slice.  in_fmt 1 ("precision mode 1"): tri-plane operands: a0 = fp16(x * 2^ea), a1 = e4m3 of
  *   the fp16 residual * 2^6, a2 = e4m3(x * 2^ea * 2^-5); w0 = fp16(w * 2^ew), w1 = e4m3(w * 2^ew *
  *   2^-6), w2 = e4m3 of the residual * 2^5.  X.W * 2^(ea+ew) = a0.w0 + a1.w1 + a2.w2: one fp16
- *   product plus two FP8 products (kind::f8f6f4, twice the rate), 2 tensor-work units per MAC.
+ *   product plus two FP8 products (e4m3 wgmma, twice the rate), 2 tensor-work units per MAC.
  * out_mode 0 / 2: split-bf16 (out0, out1); 1: fp32 (out0); 4 / 5: tri-plane activation (out0 fp16,
  *   out1 residual, out2 copy) with scale out_scale = 2^e; 2 and 5 fuse the 2x2 ceil-mode max pool.
  * acc_scale: accumulator -> true value (2^-(ea+ew) for tri-plane operands, 1 otherwise).
@@ -94,23 +94,9 @@ int mnc_roi_warp_tri(const float* feat_nhwc, int C, int H, int W, const float* r
                      float spatial_scale, float scale, void* o14_h, void* o14_l, void* o14_c,
                      void* o7_h, void* o7_l, void* o7_c, void* stream);
 
-/* Thread-block-cluster size of mnc_igemm_tc launches: 2 (default) = CTA pairs (cta_group::2): one
- * M = 256 MMA per instruction, each CTA holds its 128 pixel rows and half of the weight tile;
- * 1 = single-CTA 128-row tiles. */
-int mnc_igemm_set_cluster(int cluster_size);
-/* A/B switch: CTA pairs (cta_group::2, M = 256) in the halo kernel's precision mode 1 (default on). */
-int mnc_igemm_set_halo_pair(int on);
-/* K elements per pipeline stage: 64 (SWIZZLE_128B), 32 (SWIZZLE_64B, twice the stages) or
- * 0 = default (64; the 192-wide Cout tile always uses 32).  bn also accepts 192. */
-int mnc_igemm_set_block_k(int bk);
 /* out_mode 0 epilogue: 1 (default) = stage tiles in shared memory and write them with TMA bulk
  * tensor stores; 0 = per-thread 16-byte global stores. */
 int mnc_igemm_set_tma_store(int on);
-/* 3x3 convolutions with Cout tiles <= 128: 1 (default) = halo kernel (one TMA box of the pixel
- * tile + border feeds all 9 filter taps through shifted shared-memory descriptors);
- * 0 = per-tap activation loads. */
-int mnc_igemm_set_halo(int on);
-
 /* Same contract as mnc_igemm_tc on the fp32 SIMT pipes (exact fp32 FMA on hi+lo operands).
  * Not on the product path: it is the on-device cross-check for the tensor-core kernel. */
 int mnc_igemm_simt(const void* a_hi, const void* a_lo, int batch, int H, int W, int Cin,
@@ -251,19 +237,18 @@ int mnc_detect_tail(const float* rois, const float* rois_ext, const float* mask,
  */
 int mnc_roi_warp_nchw(const float* feat, int C, int H, int W, const float* rois, int R,
                       int pooled_h, int pooled_w, float spatial_scale, float* out, void* stream);
-/* ROIWarping 28x28 / 14x14 kernel choice (all bit-identical; scripts/gpu_roi_stage_ab.py measures them):
+/* ROIWarping 28x28 / 14x14 kernel choice (all bit-identical):
  * 2 (default) = row walk (a warp per output plane keeps the two live feature rows in registers:
  * ~1.5 loads per output); 1 = RoI window staged in shared memory (28x28 only; 4-byte cp.async,
- * channel pairs interleaved, packed fp32x2 arithmetic); 0 = per-tap gathers through L1 (round-1
+ * channel pairs interleaved, pairwise un-fused fp32 arithmetic); 0 = per-tap gathers through L1 (round-1
  * kernel; other pooled sizes always use it).  Returns the previous value. */
 int mnc_roi_warp_set_stage(int on);
 /* Launch shape of the row-walk kernel: threads per CTA (multiple of 32, <= 256) and channels per
- * CTA (default 128 / 32: every warp of the CTA owns planes; scripts/gpu_roi_walk_shape_ab.py). */
+ * CTA (default 128 / 32: every warp of the CTA owns planes). */
 int mnc_roi_warp_set_walk_shape(int threads, int channels_per_cta);
 int mnc_roi_warp_set_walk_planes14(int planes);   /* 14x14 row walk: planes per lane, 4 (default) or 8 */
 /* Fused engine form (mnc_roi_warp_split / mnc_roi_warp_tri): 0 (default) = per-cell gathers,
- * 1 = row walk (bit-identical outputs, 2.5x fewer loads, measured no faster:
- * scripts/gpu_roi_rows_ab.py).  Returns the previous value. */
+ * 1 = row walk (bit-identical outputs, 2.5x fewer loads, no faster).  Returns the previous value. */
 int mnc_roi_warp_set_rows(int on);
 int mnc_mask_resize_nchw(const float* in, int N, int C, int in_h, int in_w, int out_h, int out_w,
                          float* out, void* stream);
@@ -276,8 +261,8 @@ int mnc_roi_warp_split(const float* feat_nhwc /* fp32 [B][H][W][C] */, int C, in
                        void* o14_lo, void* o7_hi, void* o7_lo, void* stream);
 /* Kernel choice for mnc_roi_warp_split: 0 (default) = one gather of 4 taps per sample, 1 =
  * column-walking kernel (separable bilinear, taps cached in registers; 2.4x fewer loads but
- * measured 1.2-1.5x slower: serial dependence per thread, scripts/gpu_roi_warp_ab.py).  Returns the previous setting.
- * For A/B measurement (scripts/microbench.py). */
+ * slower: serial dependence per thread).  Returns the previous setting.
+ * For A/B measurement (bench.py's `micro`). */
 int mnc_roi_warp_set_walk(int on);
 int mnc_sigmoid_mask_resize(const float* logits, int stride, int R, int mask_size, int out_size,
                             float* mask_proposal, float* mask_resized, void* stream);
@@ -324,7 +309,7 @@ int mnc_mv_device(const float* boxes, const float* masks, int nb, int box_dim, i
 int mnc_mv_set_two_pass(int on);
 int mnc_mv_device_launches(void);
 /* A/B knob: pixel stride of the coarse pass and CTAs per result of the coarse / border pass
- * (defaults 6, 2, 16: the best of the shapes measured, scripts/gpu_mv_shape_ab.py). */
+ * (defaults 6, 2, 16). */
 int mnc_mv_set_shape(int stride, int chunks_coarse, int chunks_border);
 
 /* ---------------------------------------------------------------------------------------------

@@ -34,8 +34,7 @@ c_ll = ctypes.c_longlong
 c_float = ctypes.c_float
 
 
-# kernels launched by each C-ABI entry point (for bench.py's `gpu_launches` claim; checked against
-# the ncu launch list of a bench step, profiles/r02c_launches.csv).  Entry points whose kernel count
+# kernels launched by each C-ABI entry point (for bench.py's `gpu_launches` claim).  Entry points whose kernel count
 # depends on their arguments report it themselves (`launches=`: mnc_nms_sorted_launches,
 # mnc_mv_device_launches).
 launch_count = 0

@@ -387,7 +387,7 @@ __global__ void split_to_f32_kernel(const __nv_bfloat16* __restrict__ in_hi,
     out[i] = bf2f(in_hi[i]) + bf2f(in_lo[i]);
 }
 
-static inline int grid_for(long long n, int block, int cap = 148 * 16) {
+static inline int grid_for(long long n, int block, int cap = 132 * 16) {
   long long g = (n + block - 1) / block;
   if (g > cap) g = cap;
   if (g < 1) g = 1;
@@ -445,7 +445,7 @@ extern "C" int mnc_maxpool2x2_split(const void* in_hi, const void* in_lo, int ba
                                     int C, void* out_hi, void* out_lo, void* stream) {
   if (C % 8 != 0) return MNC_ERR_ARG;
   const long long total = static_cast<long long>(batch) * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8);
-  maxpool2x2_split_kernel<<<grid_for(total, 256, 148 * 32), 256, 0,
+  maxpool2x2_split_kernel<<<grid_for(total, 256, 132 * 32), 256, 0,
                             static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), batch, H,
       W, C, static_cast<__nv_bfloat16*>(out_hi), static_cast<__nv_bfloat16*>(out_lo));

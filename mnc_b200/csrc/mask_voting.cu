@@ -628,9 +628,9 @@ extern "C" int mnc_mv_set_two_pass(int on) {
 }
 extern "C" int mnc_mv_device_launches() { return g_mv_two_pass ? 5 : 4; }
 
-// launch shape of the two passes (A/B knob, scripts/gpu_mv_shape_ab.py): stride of the coarse pass,
+// launch shape of the two passes (A/B knob): stride of the coarse pass,
 // CTAs per result of the coarse / the exact border pass
-static int g_mv_stride = 6, g_mv_chunks1 = 2, g_mv_chunks2 = 16;   // measured best of 12 shapes (profiles/r02e_mv_shape_roi14_ab.json)
+static int g_mv_stride = 6, g_mv_chunks1 = 2, g_mv_chunks2 = 16;
 extern "C" int mnc_mv_set_shape(int stride, int chunks_coarse, int chunks_border) {
   if (stride < 1 || stride > 64 || chunks_coarse < 1 || chunks_border < 1 || chunks_coarse > 1024 ||
       chunks_border > 1024)

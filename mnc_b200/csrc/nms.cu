@@ -296,8 +296,7 @@ nms_lazy_kernel(const float* __restrict__ boxes, int box_stride, long long probl
 }
 
 // The same walk spread over a thread-block CLUSTER of 8 CTAs (8 SMs) per problem: phase A is
-// compute-bound on one SM (64 x kept pair tests per block; 349 us for 8 x 6000 -> 300 with heavy
-// suppression, profiles/r02c_launches_summary.txt), so each CTA tests the block's 64 candidates
+// compute-bound on one SM (64 x kept pair tests per block), so each CTA tests the block's 64 candidates
 // against every 8th part of the kept list and builds 8 of the 64 diagonal rows; the suppression
 // bits are OR-ed into, and the diagonal words stored to, EVERY CTA's shared memory through
 // distributed shared memory (double-buffered by block parity), one cluster barrier publishes them,
@@ -406,8 +405,8 @@ nms_lazy_cluster_kernel(const float* __restrict__ boxes, int box_stride, long lo
   }
 }
 
-// 256 candidates per round instead of 64 (mode 3).  The 64-candidate cluster form spends ~2 us per
-// round, most of it in the cluster barrier (a GPU-scope fence) and the hand-over to the serial
+// 256 candidates per round instead of 64 (mode 3).  The 64-candidate cluster form spends most of a
+// round in the cluster barrier (a GPU-scope fence) and the hand-over to the serial
 // resolve -- 94 rounds for 6000 candidates; with 256-candidate rounds there are 24.  One thread per
 // candidate (256 threads per CTA, 8 suppression words per row): each CTA tests all 256 candidates
 // against every 8th kept box and builds 32 of the 256 diagonal rows (warps whose candidates all
@@ -603,7 +602,7 @@ bitonic_sort_desc_kernel(const float* __restrict__ keys, long long outer_stride,
 // Top-k selection + sort, one CTA per problem: order[prob][0..min(n_valid, k)) = indices of the k
 // best entries in (key desc, index asc) order -- all that `scores.argsort()[::-1][:pre_nms_topN]`
 // (proposal_layer.py:139-142) ever uses.  Sorting all 21546 anchors (32768-slot bitonic network,
-// every stage through shared memory) cost 0.38 ms per batch; here
+// every stage through shared memory) is far more work; here
 //   1. keys -> order-preserving u32 in shared memory,
 //   2. 4-pass byte-wise radix select finds T = the k-th largest key,
 //   3. entries above T are compacted (any order), entries equal to T are taken in index order
@@ -978,7 +977,7 @@ extern "C" int mnc_nms_host(int* keep_out, int* num_out, const float* boxes_host
 // column 4) in host memory -> indices of the kept rows, in score order.  The sort
 // (`scores.argsort()[::-1]`, ties by ascending index), the gather, the NMS and the greedy scan all
 // run on the device; the host sees one H2D of the dets and one D2H of the order + keep lists
-// (the numpy sort + fancy indexing of the .pyx wrapper were most of the drop-in's 12-35 ms).
+// (the numpy sort + fancy indexing of the .pyx wrapper would otherwise dominate the drop-in).
 extern "C" int mnc_gpu_nms_host(int* keep_out, int* num_out, const float* dets_host, int n, int dim,
                                 float nms_overlap_thresh, int device_id) {
   if (n < 0 || dim < 5 || !keep_out || !num_out) return MNC_ERR_ARG;

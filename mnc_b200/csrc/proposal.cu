@@ -183,7 +183,7 @@ __global__ void stage_bridge_kernel(const float* __restrict__ rois,
 // the exponentials are evaluated in parallel, and the denominator is accumulated in COLUMN ORDER
 // -- the order of the reference's channel-sum loop -- by every lane from shuffled values, so the
 // result equals the one-thread-per-row evaluation bit for bit while the 4 launches per step drop
-// from ~16 us (a serial chain of dependent global accesses) to launch latency.
+// from a serial chain of dependent global accesses to launch latency.
 __global__ void __launch_bounds__(128)
 softmax_rows_kernel(const float* __restrict__ in, int in_stride, int rows, int cols,
                     float* __restrict__ out, int out_stride) {

@@ -1,6 +1,7 @@
-// Thin inline-PTX wrappers for the sm_100a features the MNC hot path uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld).
-// Hand-written for sm_100a only; there is no fallback path.
+// Thin inline-PTX wrappers for the sm_90a features the MNC hot path uses:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA, operands in shared memory,
+// fp32 accumulators in registers), setmaxnreg.
+// Hand-written for sm_90a only; there is no fallback path.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -21,11 +22,6 @@ __device__ __forceinline__ void fence_barrier_init() {
 }
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -50,36 +46,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void prefetch_tmap(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const void* tmap, uint64_t* bar,
-                                            int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, uint64_t* bar,
-                                            int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// Multicast variant: the box lands at the same CTA-relative offset in every CTA of `cta_mask`,
-// and complete_tx is signalled on the mbarrier at the same offset in each of them.
-__device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const void* tmap, uint64_t* bar,
-                                                  int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      ".multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
 
 // TMA store (shared -> global), bulk-group completion.
 __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* smem_src, int c0, int c1,
@@ -100,203 +66,13 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// ------------------------------------------------------------------ clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-// shared::cluster address of `smem_addr` (a shared::cta address of this CTA) in CTA `rank`.
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-// arrive on an mbarrier given by its shared::cluster address (possibly in the peer CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  // default semantics (release at CTA scope): a .release.cluster arrive compiles to
-  // MEMBAR.ALL.GPU + ERRBAR, which was 18 % of the halo pair kernel's issue-stall samples (r02 ncu).
-  // The arrive only tells the leader's MMA warp that TMEM reads have completed (ordered by
-  // tcgen05.wait::ld + tcgen05.fence::before_thread_sync); no memory is handed over.
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-
-// ------------------------------------------------------------------ CTA pair (cta_group::2)
-// Two CTAs of a cluster on one TPC execute ONE M = 256 MMA: CTA r supplies rows [128r, 128r+128)
-// of A and rows [N/2 * r, N/2 * (r+1)) of B from the same offsets of its own shared memory and
-// receives its 128 accumulator rows in its own TMEM.  Only the leader (rank 0) issues; both load.
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// TMA loads whose completion bytes are counted on the LEADER's mbarrier (`bar_cluster` = its
-// shared::cluster address); the data lands in the executing CTA's own shared memory.
-__device__ __forceinline__ void tma_load_4d_2sm_w(void* smem_dst, const void* tmap,
-                                                  uint32_t bar_cluster, int c0, int c1, int c2,
-                                                  int c3) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];\n\t}"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm_w(void* smem_dst, const void* tmap,
-                                                  uint32_t bar_cluster, int c0, int c1) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];\n\t}"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_cluster), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2sm_w(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                  uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f8_ss_2sm_w(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit of the pair's MMAs: arrives on the barrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm_w(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate, single CTA.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread retire.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// Same, arriving on the barrier at this offset in every CTA of `cta_mask`.
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i = lane i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // ------------------------------------------------------------------ warp-convergent issue
-// tcgen05.mma / tcgen05.commit / cp.async.bulk.tensor take their operands from UNIFORM registers.
-// When the issuing code sits inside `if (lane == 0) { ... }` the compiler treats every value in
-// that region as per-thread and wraps each instruction in an ELECT + 5x R2UR + branch "waterfall"
-// (~40 issue cycles per MMA, measured as the per-instruction overhead of the small-N layers).
-// The `_w` forms below are meant to be executed by ALL 32 lanes of a converged warp with
-// warp-uniform arguments: the election happens inside the asm block, so the operands are computed
-// on the uniform datapath and reach the instruction directly.  elect.sync with a full mask always
-// elects the same lane, so the MMAs and the commits that track them come from one thread.
-__device__ __forceinline__ void umma_bf16_ss_w(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_w(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast_w(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t}"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
+// cp.async.bulk.tensor takes its operands from UNIFORM registers.  When the issuing code sits
+// inside `if (lane == 0) { ... }` the compiler treats every value in that region as per-thread
+// and wraps each instruction in an election + R2UR + branch sequence.  The `_w` forms below are
+// meant to be executed by ALL 32 lanes of a converged warp with warp-uniform arguments: the
+// election happens inside the asm block, so the operands are computed on the uniform datapath and
+// reach the instruction directly.
 __device__ __forceinline__ void mbar_arrive_expect_tx_w(uint64_t* bar, uint32_t bytes) {
   asm volatile(
       "{\n\t.reg .pred q;\n\t"
@@ -327,162 +103,101 @@ __device__ __forceinline__ void tma_load_2d_w(void* smem_dst, const void* tmap, 
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mcast_w(void* smem_dst, const void* tmap, uint64_t* bar,
-                                                    int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "@q cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      ".multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;\n\t}"
-      ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
+
+// ------------------------------------------------------------------ register budget
+// A warpgroup hands registers back (producer) or takes more (consumers holding accumulators).
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
+template <int kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
 }
 
-// kind::f8f6f4 (dense FP8: E4M3 / E5M2 operands, one byte per element in shared memory, K = 32 per
-// instruction, fp32 accumulate in TMEM): twice the MAC rate of kind::f16.
-__device__ __forceinline__ void umma_f8_ss_w(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Same, with the descriptors passed as their 32-bit low words (14-bit start address field; the
-// caller adds 2 per 32 bytes) and the high words -- stride-byte-offset, version, swizzle mode:
-// compile-time constants -- as template arguments, so only two 32-bit values travel to the
-// uniform registers per instruction.
-template <uint32_t kHiA, uint32_t kHiB>
-__device__ __forceinline__ void umma_bf16_ss_w32(uint32_t tmem_d, uint32_t desc_a_lo,
-                                                 uint32_t desc_b_lo, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %6};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "r"(desc_a_lo), "r"(desc_b_lo), "r"(idesc), "r"(accumulate), "n"(kHiA), "n"(kHiB)
-      : "memory");
-}
-// kind::f8f6f4 flavour of umma_bf16_ss_w32 (descriptor low words + compile-time high words).
-template <uint32_t kHiA, uint32_t kHiB>
-__device__ __forceinline__ void umma_f8_ss_w32(uint32_t tmem_d, uint32_t desc_a_lo, uint32_t desc_b_lo,
-                                               uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %6};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], da, db, %3, p;\n\t}"
-      ::"r"(tmem_d),
-      "r"(desc_a_lo), "r"(desc_b_lo), "r"(idesc), "r"(accumulate), "n"(kHiA), "n"(kHiB)
-      : "memory");
-}
-// One filter tap of the halo kernel = four 16-wide k slices x {A_hi x [B_hi|B_lo] (idesc1),
-// A_lo x B_hi (idesc2)}: eight MMAs issued from ONE asm block -- one election, the three descriptor
-// low words + TMEM address + the two instruction descriptors cross into uniform registers once, the
-// per-slice descriptors are the bases + 2*kk.  `first` = 0 clears the accumulator on the very
-// first MMA.
-template <uint32_t kHiA, uint32_t kHiB>
-__device__ __forceinline__ void umma_halo_tap_w(uint32_t tmem_d, uint32_t la_hi, uint32_t la_lo,
-                                                uint32_t lb, uint32_t idesc1, uint32_t idesc2,
-                                                uint32_t first) {
-  asm volatile(
-      "{\n\t.reg .pred p, q, t;\n\t.reg .b32 x, y, z;\n\t.reg .b64 da, db;\n\t"
-      "elect.sync _|q, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      // kk = 0
-      "mov.b64 da, {%1, %7};\n\tmov.b64 db, {%3, %8};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-      "mov.b64 da, {%2, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t"
-      // kk = 1
-      "add.u32 x, %1, 2;\n\tadd.u32 y, %2, 2;\n\tadd.u32 z, %3, 2;\n\t"
-      "mov.b64 da, {x, %7};\n\tmov.b64 db, {z, %8};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "mov.b64 da, {y, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t"
-      // kk = 2
-      "add.u32 x, %1, 4;\n\tadd.u32 y, %2, 4;\n\tadd.u32 z, %3, 4;\n\t"
-      "mov.b64 da, {x, %7};\n\tmov.b64 db, {z, %8};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "mov.b64 da, {y, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t"
-      // kk = 3
-      "add.u32 x, %1, 6;\n\tadd.u32 y, %2, 6;\n\tadd.u32 z, %3, 6;\n\t"
-      "mov.b64 da, {x, %7};\n\tmov.b64 db, {z, %8};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "mov.b64 da, {y, %7};\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, t;\n\t}"
-      ::"r"(tmem_d),
-      "r"(la_hi), "r"(la_lo), "r"(lb), "r"(idesc1), "r"(idesc2), "r"(first), "n"(kHiA), "n"(kHiB)
-      : "memory");
-}
-
-// high words of the two descriptor flavours
-constexpr uint32_t kDescHiSw128 = (1024u >> 4) | (1u << 14) | (2u << 29);
-constexpr uint32_t kDescHiSw64 = (512u >> 4) | (1u << 14) | (4u << 29);
-constexpr uint32_t desc_hi_sw128_sbo(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 14) | (2u << 29); }
-constexpr uint32_t desc_hi_sw64_sbo(uint32_t sbo_bytes) { return (sbo_bytes >> 4) | (1u << 14) | (4u << 29); }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return (smem_addr & 0x3FFFFu) >> 4; }
-
-// K-major, 128-byte-swizzled operand tile (rows of 64 bf16 = 128 B, 8-row atoms of
-// 1024 B).  Field layout follows the sm_100 shared-memory matrix descriptor:
-// [0,14) addr>>4, [16,30) LBO>>4 (unused for swizzled K-major), [32,46) SBO>>4,
-// [46,48) version=1, [61,64) layout type (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1024u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Same for 64-byte rows (BLOCK_K = 32 bf16): 8-row atoms of 512 B, layout type 4 = SWIZZLE_64B.
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(512u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(4) << 61;
-  return d;
-}
-// 32-byte rows (32 FP8 or 16 fp16 elements per row): 8-row atoms of 256 B, layout type 6 = SWIZZLE_32B.
-__device__ __forceinline__ uint64_t umma_desc_sw32(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(256u >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(6) << 61;
-  return d;
-}
-// Descriptor of a K-major tile whose rows are `row_bytes` (128 / 64 / 32) long, swizzled with the
-// mode of the same width.
+// ------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor of a K-major operand tile whose rows are kRowBytes (128 / 64 /
+// 32) long and swizzled with the mode of the same width, as TMA writes them: 8-row atoms of
+// 8 * kRowBytes.  Fields: [0,14) address >> 4, [16,30) leading byte offset >> 4 (unused for
+// swizzled K-major), [32,46) stride byte offset >> 4 (between 8-row atoms), [62,64) swizzle
+// (1 = 128B, 2 = 64B, 3 = 32B).  A k slice inside the swizzle atom is addressed by advancing the
+// start address (32 bytes per slice).
 template <int kRowBytes>
-__device__ __forceinline__ uint64_t umma_desc_rows(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t wgmma_desc_rows(uint32_t smem_addr) {
   static_assert(kRowBytes == 128 || kRowBytes == 64 || kRowBytes == 32, "row width");
-  return kRowBytes == 128 ? umma_desc_sw128(smem_addr)
-                          : (kRowBytes == 64 ? umma_desc_sw64(smem_addr) : umma_desc_sw32(smem_addr));
+  constexpr uint64_t kMode = kRowBytes == 128 ? 1 : (kRowBytes == 64 ? 2 : 3);
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>(1) << 16;
+  d |= static_cast<uint64_t>((8u * kRowBytes) >> 4) << 32;
+  d |= kMode << 62;
+  return d;
 }
-// Instruction descriptor with A/B format code 0 and fp32 D, M = 128: kind::f16 reads it as fp16
-// operands, kind::f8f6f4 as E4M3 operands (same bit pattern: c_format = 1 at bit 4, formats 0).
-__host__ __device__ constexpr uint32_t umma_idesc_fmt0_m128(uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((128u >> 4) << 24);
+
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-// Instruction descriptor for kind::f16 with bf16 A/B (K-major both), fp32 D, M=128.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_m128(uint32_t n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24);
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
+__device__ __forceinline__ void wgmma_wait_all() {
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// keeps the compiler from moving uses of an accumulator across the asynchronous MMAs
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[32]) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) asm volatile("" : "+f"(d[j])::"memory");
+}
+
+// D[64 x 64, fp32 registers] (+)= A[64 x K, smem] * B[64 x K, smem]^T, both K-major.
+// Thread t of the warpgroup holds, for j = 0..7: d[4j], d[4j+1] = row 16*(t/32) + (t%32)/4,
+// columns 8j + 2*(t%4) + {0, 1}; d[4j+2], d[4j+3] = the same columns of row + 8.
+#define MNC_WGMMA_D32                                                                          \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                    \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define MNC_WGMMA_D32_OPS(d)                                                                   \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]),          \
+      "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]),  \
+      "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]),            \
+      "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),            \
+      "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// bf16 operands, K = 16 per instruction.
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b,
+                                               uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " MNC_WGMMA_D32
+      ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : MNC_WGMMA_D32_OPS(d)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// fp16 operands, K = 16 per instruction.
+__device__ __forceinline__ void wgmma_f16_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b,
+                                              uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " MNC_WGMMA_D32
+      ", %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : MNC_WGMMA_D32_OPS(d)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+// E4M3 operands (one byte per element in shared memory), K = 32 per instruction: twice the MAC
+// rate of the 16-bit kinds.
+__device__ __forceinline__ void wgmma_e4m3_n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b,
+                                               uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 " MNC_WGMMA_D32
+      ", %32, %33, p, 1, 1;\n\t}"
+      : MNC_WGMMA_D32_OPS(d)
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+#undef MNC_WGMMA_D32
+#undef MNC_WGMMA_D32_OPS
 
 }  // namespace ptx
 }  // namespace mnc

@@ -96,7 +96,7 @@ constexpr int kMaxPooled = 32;   // pooled_h, pooled_w <= 32
 // formed first, as roi_warping_layer.cu:56 does).  The channel loop is then 4 read-only gathers
 // (a RoI's window of one channel is <= 9.6 KB, L1-resident after first touch) + 7 un-fused fp32
 // ops per output and one vector streaming store per EPT outputs: ~13 instructions per output
-// instead of ~50 when offsets and weights are recomputed per element (profiles/README.md).
+// instead of ~50 when offsets and weights are recomputed per element.
 // Output bytes are written exactly once, coalesced (the reference also writes argmax_h/argmax_w).
 template <int PH, int PW, int EPT>
 __global__ void __launch_bounds__(256)
@@ -176,40 +176,23 @@ roi_warp_nchw_kernel(const float* __restrict__ feat, int C, int H, int W,
 // CHANNEL-PAIR INTERLEAVED: one 8-byte LDS returns a tap of two channels.  Every thread owns 4
 // consecutive outputs of the 28 x 28 plane with their window offsets and bilinear weights in
 // registers (weights formed first, products summed left to right: the operation order of
-// roi_warping_layer.cu:56) and walks the channel pairs with PACKED fp32x2 arithmetic
-// (__fmul2_rn / __fadd2_rn: two IEEE operations per instruction, no FMA contraction -- still
-// bit-exact with the reference built with -fmad=false): 4 LDS.64 + 7 packed ops per TWO outputs
-// instead of 4 LDG + 7 ops per output, one 16-byte streaming store per 4 outputs.  3.2 x fewer
-// instructions per output than the gather kernel; the window is read once from L2 instead of
+// roi_warping_layer.cu:56) and walks the channel pairs with pairwise fp32 arithmetic
+// (__fmul_rn / __fadd_rn on channel pairs: separately rounded, no FMA contraction -- still
+// bit-exact with the reference built with -fmad=false): 4 LDS.64 per TWO outputs
+// instead of 4 LDG per output, one 16-byte streaming store per 4 outputs.
+// The window is read once from L2 instead of
 // ~7 times through L1.
 constexpr int kStageGroup = 16;            // channels per CTA
 constexpr int kStageFloats = 12 * 1024;    // 48 KB window budget
 
-// Packed fp32x2 arithmetic WITHOUT fusion.  sm_100 has FMUL2 and FFMA2 but no packed add, and
-// ptxas folds every mul.rn.f32x2 -> add.rn.f32x2 (or fma by a literal 1.0) chain into one FFMA2 --
-// a single rounding, which would break bit-exactness with the reference's separately rounded
-// products and sums (measured: -fmad=false does not stop it).  So the products are FMUL2 and each
-// sum is fma(p, one, acc) with `one` = 1.0f handed in as a KERNEL ARGUMENT: p * 1.0 is exact, the
-// fma rounds once = an IEEE add, and the compiler cannot see the value, so nothing is folded.
+// Pairwise fp32 arithmetic WITHOUT fusion.  sm_90a has no packed fp32x2 instructions, so a pair is
+// two scalar operations; __fmul_rn / __fadd_rn are never contracted into an FMA, which keeps every
+// product and sum separately rounded -- bit-exact with the reference built with -fmad=false.
 __device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
-  float2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\t"
-      "mul.rn.f32x2 rc, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rc;\n\t}"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y));
-  return r;
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
 }
-__device__ __forceinline__ float2 add2_rn(float2 a, float2 b, float one) {
-  float2 r;
-  asm("{\n\t.reg .b64 ra, rb, rc, ro;\n\t"
-      "mov.b64 ra, {%2, %3};\n\tmov.b64 rb, {%4, %5};\n\tmov.b64 ro, {%6, %6};\n\t"
-      "fma.rn.f32x2 rc, rb, ro, ra;\n\t"
-      "mov.b64 {%0, %1}, rc;\n\t}"
-      : "=f"(r.x), "=f"(r.y)
-      : "f"(a.x), "f"(a.y), "f"(b.x), "f"(b.y), "f"(one));
-  return r;
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
 
 // One staged pass of NP channel pairs: window layout [pixel][S] float2 with S = NP + 1 (the odd
@@ -218,7 +201,7 @@ __device__ __forceinline__ float2 add2_rn(float2 a, float2 b, float one) {
 template <int NP>
 __device__ __forceinline__ void warp28_pass(const float2* __restrict__ win2, const int (&off)[4][4],
                                             const float2 (&wgt)[4][4], const bool (&ok)[4],
-                                            float* __restrict__ o, int n_c, float one) {
+                                            float* __restrict__ o, int n_c) {
   constexpr int S = NP + 1, PP = 28 * 28;
   const float2* t[4][4];
 #pragma unroll
@@ -232,9 +215,9 @@ __device__ __forceinline__ void warp28_pass(const float2* __restrict__ win2, con
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       float2 val = mul2_rn(wgt[e][0], t[e][0][p]);
-      val = add2_rn(val, mul2_rn(wgt[e][1], t[e][1][p]), one);
-      val = add2_rn(val, mul2_rn(wgt[e][2], t[e][2][p]), one);
-      val = add2_rn(val, mul2_rn(wgt[e][3], t[e][3][p]), one);
+      val = add2_rn(val, mul2_rn(wgt[e][1], t[e][1][p]));
+      val = add2_rn(val, mul2_rn(wgt[e][2], t[e][2][p]));
+      val = add2_rn(val, mul2_rn(wgt[e][3], t[e][3][p]));
       v[e] = ok[e] ? val : make_float2(0.f, 0.f);
     }
     __stcs(reinterpret_cast<float4*>(o + 2 * p * PP), make_float4(v[0].x, v[1].x, v[2].x, v[3].x));
@@ -245,8 +228,7 @@ __device__ __forceinline__ void warp28_pass(const float2* __restrict__ win2, con
 
 __global__ void __launch_bounds__(256)
 roi_warp28_stage_kernel(const float* __restrict__ feat, int C, int H, int W,
-                        const float* __restrict__ rois, float spatial_scale, float* __restrict__ out,
-                        float one) {
+                        const float* __restrict__ rois, float spatial_scale, float* __restrict__ out) {
   constexpr int P = 28, PP = P * P, EPT = 4, TPC = PP / EPT;   // 196 threads compute
   extern __shared__ float2 win2[];                             // [pixel][pairs + 1] (2 channels)
   __shared__ AxisTap tap_h[P], tap_w[P];
@@ -341,10 +323,10 @@ roi_warp28_stage_kernel(const float* __restrict__ feat, int C, int H, int W,
     __syncthreads();
     if (q < TPC) {
       float* o = obase + cb * PP;
-      if (np == 8) warp28_pass<8>(win2, off, wgt, ok, o, n_c, one);
-      else if (np == 4) warp28_pass<4>(win2, off, wgt, ok, o, n_c, one);
-      else if (np == 2) warp28_pass<2>(win2, off, wgt, ok, o, n_c, one);
-      else warp28_pass<1>(win2, off, wgt, ok, o, n_c, one);
+      if (np == 8) warp28_pass<8>(win2, off, wgt, ok, o, n_c);
+      else if (np == 4) warp28_pass<4>(win2, off, wgt, ok, o, n_c);
+      else if (np == 2) warp28_pass<2>(win2, off, wgt, ok, o, n_c);
+      else warp28_pass<1>(win2, off, wgt, ok, o, n_c);
     }
     __syncthreads();
   }
@@ -362,7 +344,7 @@ roi_warp28_stage_kernel(const float* __restrict__ feat, int C, int H, int W,
 // Stores: one 4 x P byte row segment per sample row, consecutive rows contiguous (whole plane
 // written once, streaming).  P = 14 packs two planes into one warp (lanes 0-13 and 16-29).
 template <int P, int CH = ((P > 16) ? 8 : 4)>   // CH: planes walked together by one lane (ILP; the row
-                                                // bookkeeping and the 4 weights are shared; measured)
+                                                // bookkeeping and the 4 weights are shared)
 __global__ void __launch_bounds__(256)
 roi_warp_rowwalk_kernel(const float* __restrict__ feat, int C, int H, int W,
                         const float* __restrict__ rois, float spatial_scale, int ch_per_cta,
@@ -701,7 +683,7 @@ roi_warp_split_kernel(const float* __restrict__ feat, int C, int H, int W,
 // rows at that column's two taps in registers, and re-reads only when the row taps move on
 // (bin_h < 1.4 feature rows per sample row): ~4*SUB loads per NEW FEATURE ROW instead of 4*SUB*SUB
 // per pooled cell -- 2.5x fewer 16-byte loads through L1 for a typical proposal (the gather form
-// is L1-bandwidth bound: l1tex 94 %, r02 ncu).  Same 4-tap formula as the gather form (weights
+// is L1-bandwidth bound).  Same 4-tap formula as the gather form (weights
 // first, FMA chain).  The 2x2 pooling to 7x7 pairs neighbouring columns by one warp shuffle.
 // grid (R, C/64), 224 threads = 7 warps x (2 columns x 16 channel quads).
 template <int SUB, bool TRI, int NQ>
@@ -1155,7 +1137,7 @@ static inline int grid_for(long long n, int block, int cap) {
 
 using namespace mnc;
 
-static int g_roi_stage = 2;   // 2: row walk (default, fastest measured); 1: staged window; 0: gather
+static int g_roi_stage = 2;   // 2: row walk (default); 1: staged window; 0: gather
 extern "C" int mnc_roi_warp_set_stage(int on) {
   const int prev = g_roi_stage;
   g_roi_stage = on;   // 0: gather kernel, 1: shared-memory staged window (28x28), 2: row walk
@@ -1205,13 +1187,13 @@ extern "C" int mnc_roi_warp_nchw(const float* feat, int C, int H, int W, const f
       roi_warp_rowwalk_kernel<14><<<wgrid, threads, 0, s>>>(feat, C, H, W, rois, spatial_scale, cpc, out);
     return check_launch();
   }
-  // (14x14: 784 taps per channel against a ~440-float window -- staging does not pay, measured)
+  // (14x14: 784 taps per channel against a ~440-float window -- staging does not pay)
   if (stage && g_roi_stage == 1 && pooled_h == 28 && pooled_w == 28) {
     dim3 sgrid(R, (C + kStageGroup - 1) / kStageGroup);
     static SmemGrant grant28;
     const int smem = kStageFloats * 4;
     if (!ensure_dynamic_smem(roi_warp28_stage_kernel, smem, grant28)) return MNC_ERR_CUDA;
-    roi_warp28_stage_kernel<<<sgrid, 256, smem, s>>>(feat, C, H, W, rois, spatial_scale, out, 1.0f);
+    roi_warp28_stage_kernel<<<sgrid, 256, smem, s>>>(feat, C, H, W, rois, spatial_scale, out);
     return check_launch();
   }
   if (pooled_h == 28 && pooled_w == 28)
@@ -1230,7 +1212,7 @@ extern "C" int mnc_mask_resize_nchw(const float* in, int N, int C, int in_h, int
                                     int out_w, float* out, void* stream) {
   const long long total = static_cast<long long>(N) * C * out_h * out_w;
   if (total <= 0) return MNC_OK;
-  mask_resize_nchw_kernel<<<grid_for(total, 256, 148 * 8), 256, 0,
+  mask_resize_nchw_kernel<<<grid_for(total, 256, 132 * 8), 256, 0,
                             static_cast<cudaStream_t>(stream)>>>(in, N * C, in_h, in_w, out_h,
                                                                  out_w, out);
   return check_launch();
@@ -1245,23 +1227,23 @@ extern "C" int mnc_mask_pool_nchw(const float* feat, const float* mask, int N, i
                    ((reinterpret_cast<uintptr_t>(mask) & 15) == 0) &&
                    ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
   if (vec)
-    mask_pool_nchw_kernel<<<grid_for(total / 4, 256, 148 * 16), 256, 0,
+    mask_pool_nchw_kernel<<<grid_for(total / 4, 256, 132 * 16), 256, 0,
                             static_cast<cudaStream_t>(stream)>>>(feat, mask, N, C, hw, out);
   else
-    mask_pool_nchw_scalar_kernel<<<grid_for(total, 256, 148 * 16), 256, 0,
+    mask_pool_nchw_scalar_kernel<<<grid_for(total, 256, 132 * 16), 256, 0,
                                    static_cast<cudaStream_t>(stream)>>>(feat, mask, N, C, hw, out);
   return check_launch();
 }
 
 static int g_roi_rows = 0;   // fused engine form: 0 = per-cell gathers (default), 1 = row walk (bit-identical,
-                             // 2.5x fewer loads, not faster: 0.625-0.641 vs 0.639 ms at 28x28, 0.38-0.41 vs 0.305 at 14x14:
+                             // 2.5x fewer loads, not faster:
                              // the kernel is bound by its 1.2 GB of output and the 4x sample arithmetic, not by taps)
 extern "C" int mnc_roi_warp_set_rows(int on) {
   const int prev = g_roi_rows;
   g_roi_rows = (on == 1 || on == 2) ? on : 0;   // channel quads per thread
   return prev;
 }
-static int g_roi_walk = 0;  // measured slower on real proposals (profiles/README.md): latency-bound
+static int g_roi_walk = 0;  // slower on real proposals: latency-bound
 extern "C" int mnc_roi_warp_set_walk(int on) {
   const int prev = g_roi_walk;
   g_roi_walk = on ? 1 : 0;

@@ -109,7 +109,7 @@ mask_pool_tri_kernel(const __half* __restrict__ f_h, const uint8_t* __restrict__
 
 static inline int tri_grid(long long n, int block) {
   long long g = (n + block - 1) / block;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (g < 1) g = 1;
   return static_cast<int>(g);
 }

@@ -227,26 +227,6 @@ def igemm(a, batch, H, W, cin, w, cout, taps, bias=None, relu=False, out=None, o
         check(rc, "mnc_igemm_simt")
 
 
-cluster_size = 2      # CTAs per work item of igemm_tc_kernel (tracked for the engine's split-K model)
-
-
-def set_cluster(cl):
-    """Thread-block-cluster size of the tensor-core launches (1 or 2, default 2)."""
-    global cluster_size
-    check(lib.mnc_igemm_set_cluster(c_int(cl)), "mnc_igemm_set_cluster")
-    cluster_size = cl
-
-
-def set_halo_pair(on):
-    """A/B: CTA pairs in the halo kernel's precision mode 1 (default on)."""
-    check(lib.mnc_igemm_set_halo_pair(c_int(int(on))), "mnc_igemm_set_halo_pair")
-
-
-def set_block_k(bk):
-    """K elements per pipeline stage of the tensor-core launches: 64, 32 or 0 (= per-shape default)."""
-    check(lib.mnc_igemm_set_block_k(c_int(bk)), "mnc_igemm_set_block_k")
-
-
 def splitk_reduce(partial, splits, split_stride, rows, cols, bias=None, relu=False, out=None,
                   out_f32=None, out_row_stride=None, out_ch_offset=0):
     if out_f32 is not None:

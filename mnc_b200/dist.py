@@ -2,7 +2,7 @@
 
 The path shards naturally: images are independent (the reference is batch-1 and has no
 cross-image op; SURVEY.md section 8e), so there is no collective inside the forward.  One process
-per GPU (`torch.distributed`, NCCL over NVLink/NVSwitch on the B200 box; gloo in the CPU tests);
+per GPU (`torch.distributed`, NCCL over NVLink/NVSwitch; gloo in the CPU tests);
 weights are replicated; the only exchange is a single all-gather of fixed-size records:
     [count | boxes 600x4 | scores 600x21 | masks 600x441]  fp32  (~1.12 MB per image).
 """

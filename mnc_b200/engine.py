@@ -8,8 +8,8 @@ times per image for its Python layers: SURVEY.md section 3.2).  The reference is
 image on device and stacking RoIs with their batch index (ROIWarping honours roi[0],
 roi_warping_layer.cu:79,96), so the FC weights stream from HBM once per batch.
 
-PyTorch's role: device memory and streams (a step is ~60 asynchronous launches queued in 1.2 ms
-of host time against 15 ms of device time, so no CUDA graph is needed to keep the GPU busy).  Apart
+PyTorch's role: device memory and streams (a step is ~60 asynchronous launches, queued in far less host
+time than they take on the device).  Apart
 from a few `torch.cat` / copies in the `detect` tail, no torch op computes on the path.
 """
 import math
@@ -31,22 +31,16 @@ def _ceil_half(x):
     return (x + 1) // 2
 
 
-HALO_MAX_COUT = 128    # 3x3 convs with Cout <= 128 run the halo kernel
-
-
-def pick_split_k(tiles_m, tiles_n, k_steps, sms, cluster=2, max_split=32, out_elems=0):
+def pick_split_k(tiles_m, tiles_n, k_steps, sms, max_split=32, out_elems=0):
     """Split-K only when the launch cannot fill the GPU (e.g. fc6_maskest: 19 row tiles,
-    K = 100352; every FC at batch 1).  A wave-quantisation-driven split (608 tiles -> 4.1 waves)
-    was measured and rejected: the extra fp32 partial reduce costs what the shorter tail saves
-    (profiles/README.md).  When splitting, the factor minimises waves x k-steps-per-item, counted
-    the way the kernel schedules: a work item is a CTA PAIR (two adjacent 128-row tiles x one
-    Cout tile x one split) and there are sms/2 of them in flight (igemm_tc.cu launch_igemm).
-    (Counting single tiles against 148 SMs picked 15 splits for fc6_maskest = 150 items = three
-    waves of 74, the last with 2 items; and 2 splits for fc6 at batch 1 = 88 items = two waves,
-    i.e. no gain at all.)  Cost unit: one k-step of a pair item (~0.45 us); each split adds a
-    launch-side constant and one fp32 copy of the output to write and re-read (M*N*8 B at ~5 TB/s)."""
-    slots = max(1, sms // cluster)
-    items = math.ceil(tiles_m / cluster) * tiles_n
+    K = 100352; every FC at batch 1).  When splitting, the factor minimises waves x
+    k-steps-per-item, counted the way the kernel schedules: a work item is one 128-row tile x one
+    Cout tile x one split, and one persistent CTA per SM takes them in turn (igemm_tc.cu
+    launch_igemm).  Cost unit: one k-step of an item; each split adds a launch-side constant and
+    one fp32 copy of the output to write and re-read
+    (the constants below were fitted on another GPU and have not been re-measured on the H100)."""
+    slots = max(1, sms)
+    items = tiles_m * tiles_n
     if items >= slots * 0.7 or k_steps < 16:
         return 1
     per_split = 0.5 + out_elems * 1.7e-6
@@ -62,11 +56,9 @@ def pick_split_k(tiles_m, tiles_n, k_steps, sms, cluster=2, max_split=32, out_el
 class MNCEngine:
     # "f16f8": precision mode 1 on every launch of the per-tap / inner-product kernel -- tri-plane
     # operands, fp16 main product + two FP8 correction products (2 tensor-work units per MAC);
-    # "bf16x3": split-bf16 operands everywhere (3 units per MAC).  The halo kernel (Cout <= 128)
-    # has both modes as well (HALO_TRI False keeps it on split-bf16 operands under "f16f8");
+    # "bf16x3": split-bf16 operands everywhere (3 units per MAC);
     # conv1_1 (K = 27) computes in split bf16 in both and writes the format its consumer reads.
     DEFAULT_PRECISION = "f16f8"
-    HALO_TRI = True
 
     def __init__(self, weights, device="cuda", impl="tc", sm_count=None, precision=None):
         """weights: {caffe name: (weight, bias)} fp32 tensors in Caffe layouts (see weights.py)."""
@@ -74,7 +66,6 @@ class MNCEngine:
         self.impl = impl
         self.precision = (precision or self.DEFAULT_PRECISION) if impl == "tc" else "bf16x3"
         self.tri = self.precision == "f16f8"
-        self.halo_tri = self.HALO_TRI
         self.fuse_pool = True
         # per-tensor exponents of the tri-plane activations, measured on the first forward
         self.exp = {}
@@ -93,8 +84,6 @@ class MNCEngine:
         # 64-channel conv1_1 runs on the tensor cores (stacked hi/lo weight tile, K padded to 32)
         self.conv1_1_tc = (dense.conv1_1_weight_to_tc(w["conv1_1"][0])
                            if impl == "tc" and w["conv1_1"][0].shape[0] == 64 else None)
-        if self.conv1_1_tc is None:
-            self.halo_tri = False      # only the tensor-core conv1_1 writes tri-plane output
         self.convs = []
         for name in TRUNK_NAMES[1:] + ["rpn_conv_3x3"]:
             if name in w:   # the CFM test net has no RPN (proposals are an input)
@@ -225,14 +214,12 @@ class MNCEngine:
         return t[:need].view(*shape)
 
     def _linear(self, a, M, K, wgt, N, bias, relu, out=None, out_f32=None, out_stride=None,
-                out_ch_offset=0, key="lin", block_k=0, bn=0, exp_key=None):
+                out_ch_offset=0, key="lin", bn=0, exp_key=None):
         """y = act(a @ W^T + b) through the implicit-GEMM kernel; split-K when the tile count
         cannot fill the GPU (e.g. fc6_maskest: K = 100352, N = 256).  a / wgt / out: split-bf16
         tensors or dense.Tri (out written with the exponent of `exp_key`)."""
         tri_in = isinstance(a, dense.Tri)
-        # Cout tile: 192 for the wide layers -- at M = 2400, N = 4096 it gives 19 x 22 = 418 tiles
-        # (220 CTA-pair items = 2.97 waves of 74 pairs), against 2.16 (-> 3) waves at 256
-        bn = bn or (64 if N <= 64 else (128 if N <= 128 else (192 if N >= 1024 else 256)))
+        bn = bn or (64 if N <= 64 else 128)
         k_steps = K // 64
         split = (self._pick_split(math.ceil(M / 128), math.ceil(N / bn), k_steps, out_elems=M * N)
                  if self.impl == "tc" else 1)
@@ -255,13 +242,7 @@ class MNCEngine:
                 run(0, None)
             return
         part = self._f32_buf("splitk_" + key, split, M, N)
-        if block_k and not tri_in:
-            dense.set_block_k(block_k)
-        try:
-            dense.igemm2(a4, 1, 1, M, K, wgt, N, 1, out_f32=part, split_k=split, split_stride=M * N, bn=bn)
-        finally:
-            if block_k and not tri_in:
-                dense.set_block_k(0)
+        dense.igemm2(a4, 1, 1, M, K, wgt, N, 1, out_f32=part, split_k=split, split_stride=M * N, bn=bn)
         if tri_out:
             self._scaled(ek, lambda e, amax: dense.splitk_reduce_tri(
                 part, split, M * N, M, N, out, e, bias=bias, relu=relu, out_row_stride=out_stride,
@@ -272,7 +253,7 @@ class MNCEngine:
 
     def _pick_split(self, tiles_m, tiles_n, k_steps, max_split=32, out_elems=0):
         """Split-K factor of one tensor-core launch: see pick_split_k."""
-        return pick_split_k(tiles_m, tiles_n, k_steps, self.sms, dense.cluster_size, max_split, out_elems)
+        return pick_split_k(tiles_m, tiles_n, k_steps, self.sms, max_split, out_elems)
 
     def _conv(self, x, B, H, W, cin, wgt, cout, bias, out, key, pool=False):
         """3x3 conv + bias + ReLU (+ fused 2x2 ceil-mode max pool) -> `out` (split-bf16 or Tri),
@@ -280,7 +261,7 @@ class MNCEngine:
         if self.impl != "tc":
             dense.igemm(x, B, H, W, cin, wgt, cout, 9, bias=bias, relu=True, out=out, impl=self.impl)
             return
-        bn = 64 if cout <= 64 else (128 if cout <= 128 else 256)
+        bn = 64 if cout <= 64 else 128
         split = 1 if pool else self._pick_split(B * math.ceil(H / 8) * math.ceil(W / 16),
                                                 math.ceil(cout / bn), 9 * cin // 64, max_split=4,
                                                 out_elems=B * H * W * cout)
@@ -306,7 +287,7 @@ class MNCEngine:
     # ------------------------------------------------------------------ trunk
     def _conv_in_tri(self, cout):
         """Does the conv with `cout` output channels read tri-plane operands?"""
-        return self.tri and (cout > HALO_MAX_COUT or self.halo_tri)
+        return self.tri and (cout > 128 or self.conv1_1_tc is not None)
 
     def trunk(self, data):
         """conv1_1 .. conv5_3 (test.prototxt:19-387).  data fp32 (B,3,H,W) -> NHWC conv5_3 in the
@@ -385,12 +366,11 @@ class MNCEngine:
         # (not worth a fork / join for a handful of RoIs: single-image latency is launch-count bound)
         fork = self.overlap_heads and not self._calibrating and R >= 4 * ROIS_PER_IMAGE
         h_me = self._act_buf("h_me", R, me, exp_key="h_me_" + tag)
-        # fc6_maskest streams its 963 MB activation matrix from HBM exactly once (a single Cout
-        # tile: no L2 reuse), so it wants loads in flight rather than big stages (split-bf16 mode:
-        # BLOCK_K 32 gives a 4-deep ring at BN 256).  What remains (2.7 TB/s) is the DRAM efficiency
-        # of 128-byte row segments 200 KB apart, the price of K-major rows with K = 100352.
+        # fc6_maskest streams its 963 MB activation matrix from HBM exactly once; what bounds it is the
+        # DRAM efficiency of 128-byte row segments 200 KB apart, the price of K-major rows with
+        # K = 100352 (split-K items take interleaved k-steps to read adjacent segments together).
         self._linear(feat14, R, 196 * c5, self.fc6_maskest[0], me, self.fc6_maskest[1], True,
-                     out=h_me, key="me", block_k=32, exp_key="h_me_" + tag)
+                     out=h_me, key="me", exp_key="h_me_" + tag)
         logits = self._f32_buf("mask_logits_" + tag, R, 448)
         self._linear(h_me, R, me, self.mask_pred[0], 441, self.mask_pred[1], False,
                      out_f32=logits, out_stride=448, key="mp")
@@ -449,7 +429,7 @@ class MNCEngine:
 
     @staticmethod
     def _fc_bn(N):
-        return 64 if N <= 64 else (128 if N <= 128 else (192 if N >= 1024 else 256))
+        return 64 if N <= 64 else 128
 
     # ------------------------------------------------------------------ trunk + RPN + proposals
     def conv5_f32(self, conv5_3, B, H5, W5):

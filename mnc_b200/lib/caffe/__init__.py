@@ -9,7 +9,7 @@ pycaffe.py:62-108; tools/demo.py:126-129,70-90; lib/caffeWrapper/TesterWrapper.p
 
 ``Net`` does not interpret arbitrary graphs: it accepts the MNC 5-stage test graph
 (models/VGG16/mnc_5stage/test.prototxt, checked layer by layer against caffe/mnc_graph.py) and runs
-it on the fused B200 engine.  CPU mode does not exist (the reference's MNC layers are
+it on the fused engine.  CPU mode does not exist (the reference's MNC layers are
 NOT_IMPLEMENTED on CPU too: roi_warping_layer.cpp:47)."""
 from collections import OrderedDict
 

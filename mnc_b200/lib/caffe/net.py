@@ -1,4 +1,4 @@
-"""caffe.Net for the MNC 5-stage test graph, on the fused B200 engine."""
+"""caffe.Net for the MNC 5-stage test graph, on the fused engine."""
 from collections import OrderedDict
 
 import numpy as np

@@ -86,7 +86,7 @@ class CFMEngine(MNCEngine):
                      out_stride=2 * fc, out_ch_offset=0, key="fc7")
         h_me = self._split_buf("h_me", R, me)
         self._linear(feat14, R, 196 * c5, self.fc6_maskest[0], me, self.fc6_maskest[1], True,
-                     out=h_me, key="me", block_k=32)
+                     out=h_me, key="me")
         logits = self._f32_buf("mask_logits_cfm", R, 448)
         self._linear(h_me, R, me, self.mask_pred[0], 441, self.mask_pred[1], False,
                      out_f32=logits, out_stride=448, key="mp")

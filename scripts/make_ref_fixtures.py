@@ -239,6 +239,27 @@ def softmax_rows(rng, n, c, scale=1.0):
     return (e / e.sum(1, keepdims=True)).astype(np.float32)
 
 
+def save_parts(path, items, limit=900000):
+    """np.savez_compressed in as many files as it takes to keep each under `limit` bytes:
+    <name>.npz, <name>.part2.npz, ... (tests/test_ref_fixtures.py load() reads them back as one)."""
+    import io
+
+    def size(d):
+        b = io.BytesIO()
+        np.savez_compressed(b, **d)
+        return len(b.getvalue())
+    parts = [{}]
+    for k, v in items.items():
+        trial = dict(parts[-1])
+        trial[k] = v
+        if parts[-1] and size(trial) > limit:
+            parts.append({k: v})
+        else:
+            parts[-1] = trial
+    for i, d in enumerate(parts):
+        np.savez_compressed(path if i == 0 else "%s.part%d.npz" % (path[:-4], i + 1), **d)
+
+
 def main():
     native = {"nms": [], "mv": []}
     install_reference_environment(native)
@@ -350,7 +371,7 @@ def main():
                    "proposal_index_" + tag: np.asarray(layer._proposal_index)})
         meta["proposal_" + tag] = int(top[0].data.shape[0])
     pl["cases"] = np.array([c[0] for c in cases])
-    np.savez_compressed(os.path.join(OUT, "ref_proposal.npz"), **pl)
+    save_parts(os.path.join(OUT, "ref_proposal.npz"), pl)
 
     # ---- StageBridgeLayer / MaskLayer (TEST) -----------------------------------------------------
     sb = {}
@@ -427,7 +448,7 @@ def main():
             assert np.array_equal(dets, np.hstack((boxes, scores[:, c:c + 1])))
             mvf["nms_keep_%s_c%d" % (tag, c)] = keep.astype(np.int32)
         meta["voting_" + tag] = int(sum(len(b) for b in lb))
-    np.savez_compressed(os.path.join(OUT, "ref_voting.npz"), **mvf)
+    save_parts(os.path.join(OUT, "ref_voting.npz"), mvf)
 
     # ---- prep_im_for_blob / prepare_mnc_args / im_detect tail -----------------------------------
     class Net(object):
@@ -475,7 +496,7 @@ def main():
                    "out_boxes_" + tag: boxes, "out_masks_" + tag: masks, "out_scores_" + tag: scores})
         meta["tail_%s_boxes_dtype" % tag] = str(boxes.dtype)
     pr["cases"] = np.array([c[0] for c in pcases])
-    np.savez_compressed(os.path.join(OUT, "ref_prep_tail.npz"), **pr)
+    save_parts(os.path.join(OUT, "ref_prep_tail.npz"), pr)
 
     # ---- recorded native calls (replayed on the GPU box through oracle/_ref) --------------------
     # `_nms` calls made by ProposalLayer.forward (the voting ones are in ref_voting.npz as keep lists;

@@ -91,13 +91,13 @@ def test_prototxt_reader_and_graph_check(tmp_path):
     p.write_text(emit(mnc_graph.GRAPHS["cfm"](), ("data", "im_info")))
     with pytest.raises(ValueError):
         mnc_graph.identify_prototxt(str(p))           # CFM layers with the wrong inputs
-    base = "/root/reference/models/VGG16/"
-    if os.path.exists(base):  # build container only
-        assert len(mnc_graph.check_prototxt(base + "mnc_5stage/test.prototxt")) == 88
-        assert mnc_graph.identify_prototxt(base + "faster_rcnn_end2end/test.prototxt")[0] == "faster_rcnn"
-        assert mnc_graph.identify_prototxt(base + "cfm/test.prototxt")[0] == "cfm"
-        with pytest.raises(ValueError):
-            mnc_graph.identify_prototxt(base + "mnc_5stage/train.prototxt")
+    # the reference's own model files (models/VGG16/, stored under tests/golden/ref_models)
+    base = os.path.join(ROOT, "tests", "golden", "ref_models") + os.sep
+    assert len(mnc_graph.check_prototxt(base + "mnc_5stage/test.prototxt")) == 88
+    assert mnc_graph.identify_prototxt(base + "faster_rcnn_end2end/test.prototxt")[0] == "faster_rcnn"
+    assert mnc_graph.identify_prototxt(base + "cfm/test.prototxt")[0] == "cfm"
+    with pytest.raises(ValueError):
+        mnc_graph.identify_prototxt(base + "mnc_5stage/train.prototxt")
 
 
 def test_cfg_constants():
@@ -280,19 +280,18 @@ def test_hdf5_reader_on_reference_test_files_and_caffemodel_h5(tmp_path):
     B-tree spans several symbol-table nodes; (3) the engine weight dict from it."""
     from mnc_b200 import hdf5_min, weights as Wt, caffemodel as CM
     from tests.util import write_h5_tree
-    base = "/root/reference/caffe-mnc/src/caffe/test/test_data/"
-    if os.path.exists(base + "sample_data.h5"):   # build container only
-        data = np.arange(10 * 8 * 6 * 5).reshape(10, 8, 6, 5).astype(np.float32)
-        label = (1 + np.arange(10)[:, None]).astype(np.float32)
-        d = hdf5_min.read_hdf5(base + "sample_data.h5")
-        assert set(d) == {"/data", "/label", "/label2"}
-        assert np.array_equal(d["/data"], data) and np.array_equal(d["/label"], label)
-        assert np.array_equal(d["/label2"], label + 1)
-        g = hdf5_min.read_hdf5(base + "sample_data_2_gzip.h5")
-        assert np.array_equal(g["/data"], data + data.size) and g["/label"].dtype == np.uint8
-        assert np.array_equal(g["/label2"], (label + 1).astype(np.uint8))
-        s = hdf5_min.read_hdf5(base + "solver_data.h5")
-        assert s["/data"].shape == (8, 3, 10, 10) and s["/targets"].shape == (8, 1)
+    base = os.path.join(ROOT, "tests", "golden", "ref_hdf5") + os.sep   # copies of those test files
+    data = np.arange(10 * 8 * 6 * 5).reshape(10, 8, 6, 5).astype(np.float32)
+    label = (1 + np.arange(10)[:, None]).astype(np.float32)
+    d = hdf5_min.read_hdf5(base + "sample_data.h5")
+    assert set(d) == {"/data", "/label", "/label2"}
+    assert np.array_equal(d["/data"], data) and np.array_equal(d["/label"], label)
+    assert np.array_equal(d["/label2"], label + 1)
+    g = hdf5_min.read_hdf5(base + "sample_data_2_gzip.h5")
+    assert np.array_equal(g["/data"], data + data.size) and g["/label"].dtype == np.uint8
+    assert np.array_equal(g["/label2"], (label + 1).astype(np.uint8))
+    s = hdf5_min.read_hdf5(base + "solver_data.h5")
+    assert s["/data"].shape == (8, 3, 10, 10) and s["/targets"].shape == (8, 1)
     w = Wt.make_weights(Wt.TINY_ARCH)
     tree = {"data": {}, "diff": {}}
     for name, (wt, b) in w.items():
@@ -391,31 +390,30 @@ def test_sbd_ground_truth_cache(tmp_path):
     assert (cache / "bicycle_mask_gt.pkl").stat().st_mtime_ns == stamp
 
 
-def test_split_k_model_counts_cta_pair_work_items():
-    """engine.pick_split_k: the factor is chosen in the kernel's own scheduling unit (CTA-pair work
-    items on sms/2 slots, igemm_tc.cu launch_igemm), not single tiles on all SMs."""
+def test_split_k_model_counts_tiles_per_sm():
+    """engine.pick_split_k: the factor is chosen in the kernel's own scheduling unit (128-row x
+    128-column tiles taken in turn by one persistent CTA per SM, igemm_tc.cu launch_igemm) on the
+    132 SMs of an H100."""
     import math
     from mnc_b200.engine import pick_split_k
 
-    def pick(M, N, K, bn, **kw):
-        return pick_split_k(math.ceil(M / 128), math.ceil(N / bn), K // 64, 148, 2, out_elems=M * N, **kw)
+    def pick(M, N, K, bn=128, **kw):
+        return pick_split_k(math.ceil(M / 128), math.ceil(N / bn), K // 64, 132, out_elems=M * N, **kw)
 
-    def waves(M, N, bn, s):
-        return math.ceil(M / 256) * math.ceil(N / bn) * s / 74.0
+    def waves(M, N, s, bn=128):
+        return math.ceil(M / 128) * math.ceil(N / bn) * s / 132.0
 
     # launches that fill the GPU are never split (fc6 / fc7 at the benchmarked batch 8)
-    assert pick(2400, 4096, 25088, 192) == 1 and pick(2400, 4096, 4096, 192) == 1
-    # fc6_maskest at batch 8: 10 row pairs -> 7 splits = 70 items = one wave (15 was three waves)
-    s = pick(2400, 256, 100352, 256)
-    assert s == 7 and waves(2400, 256, 256, s) <= 1.0
-    # batch 1: fc6 (2 row pairs x 22 Cout tiles) -> 5 splits = 220 items = 2.97 waves
-    s = pick(300, 4096, 25088, 192)
-    assert s == 5 and 2.9 < waves(300, 4096, 192, s) <= 3.0
+    assert pick(2400, 4096, 25088) == 1 and pick(2400, 4096, 4096) == 1
+    # fc6_maskest at batch 8: 19 row tiles x 2 Cout tiles = 38 items -> split into whole waves
+    s = pick(2400, 256, 100352)
+    assert s == 10 and 2.8 < waves(2400, 256, s) <= 3.0
+    # batch 1: fc6 (3 row tiles x 32 Cout tiles = 96 items) already fills 70 % of the SMs
+    assert pick(300, 4096, 25088) == 1
     # tiny K is never split; the conv path caps the factor at 4
-    assert pick(300, 441, 256, 256) == 1
-    assert pick_split_k(20, 2, 72, 148, 2, max_split=4, out_elems=2394 * 512) <= 4
-    # single-CTA scheduling (cluster 1) keeps the old counting
-    assert pick_split_k(19, 1, 1568, 148, 1, out_elems=2400 * 256) in range(2, 33)
+    assert pick(300, 441, 256) == 1
+    assert pick_split_k(20, 2, 72, 132, max_split=4, out_elems=2394 * 512) <= 4
+    assert pick_split_k(19, 1, 1568, 132, out_elems=2400 * 256) in range(2, 33)
 
 
 def test_bench_cpu_arm_is_bounded_and_counts_usable_cores(monkeypatch):

@@ -73,7 +73,7 @@ def test_conv3x3(B, H, W, Cin, Cout, bn):
     out = torch.zeros(2, B, H, W, Cout, device="cuda", dtype=torch.bfloat16)
     dense.igemm(xs, B, H, W, Cin, ws, Cout, 9, bias=b, relu=True, out=out, bn=bn)
     assert relerr(dense.merge(out), ref) < 1e-4
-    # precision mode 1 on the same layer (per-tap kernel, CTA pairs), tri-plane in and out
+    # precision mode 1 on the same layer tri-plane in and out
     xt, wt = dense.tri_from_f32(x.permute(0, 2, 3, 1).contiguous()), dense.conv_weight_to_tri(w)
     ot = dense.tri_alloc((B, H, W, Cout), "cuda")
     dense.igemm2(xt, B, H, W, Cin, wt, Cout, 9, bias=b, relu=True, out=ot,
@@ -125,7 +125,7 @@ def test_conv1_1_tensor_core_form(B, H, W):
     simt = torch.zeros_like(out)
     dense.conv1_1(data, w, b, simt)
     assert relerr(dense.merge(out), dense.merge(simt).double()) < 1e-4
-    # tri-plane output (what the precision-mode-1 halo kernel reads) + the running max |output|
+    # tri-plane output (what the precision-mode-1 convolutions read) + the running max |output|
     ot = dense.tri_alloc((B, H, W, 64), "cuda")
     amax = torch.zeros(1, dtype=torch.int32, device="cuda")
     dense.conv1_1_tc(data, dense.conv1_1_weight_to_tc(w), b, ot, out_exp=dense.exp_for(float(ref.max())),
@@ -154,7 +154,7 @@ def test_conv3x3_with_fused_ceil_mode_pool(B, H, W, Cin, Cout, bn):
     dense.igemm(xs, B, H, W, Cin, ws, Cout, 9, bias=b, relu=True, out=pooled, bn=bn, pool=True)
     want = F.max_pool2d(dense.merge(full).permute(0, 3, 1, 2), 2, 2, ceil_mode=True).permute(0, 2, 3, 1)
     assert torch.equal(dense.merge(pooled), want)
-    # precision mode 1 (halo kernel for bn <= 128, per-tap kernel above), tri-plane in and out
+    # precision mode 1 tri-plane in and out
     if Cout % 16 != 0:     # tri-plane rows are 16-byte aligned in every plane: Cout % 16 == 0
         with pytest.raises(Exception, match="MNC_ERR_ARG"):
             dense.igemm2(dense.tri_from_f32(x.permute(0, 2, 3, 1).contiguous()), B, H, W, Cin,

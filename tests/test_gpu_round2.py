@@ -1,5 +1,5 @@
-"""Round-2 machinery on the GPU: tri-plane conversions, precision modes against each other, CTA-pair
-vs single-CTA MMAs, CUDA-graph replay vs eager launches, the pipelined host API."""
+"""Tri-plane conversions, precision modes against each other and against fp64, CUDA-graph replay
+vs eager launches, the pipelined host API."""
 import numpy as np
 import pytest
 import torch
@@ -30,9 +30,9 @@ def test_tri_conversion_device_equals_torch_restatement():
 
 
 @pytest.mark.parametrize("M,N,K", [(300, 256, 512), (2400, 192, 4096), (257, 448, 1024)])
-def test_pair_and_single_cta_agree_in_both_modes(M, N, K):
-    """CTA-pair (cta_group::2, M = 256) and single-CTA launches accumulate the same products in the
-    same order: bit-identical; precision mode 1 stays within 3e-5 of fp64 like the split-bf16 mode."""
+def test_both_precision_modes_match_fp64(M, N, K):
+    """Inner product in both operand formats: precision mode 1 stays within 3e-5 of fp64 like the
+    split-bf16 mode, and a second launch on the same operands returns the same bits."""
     from mnc_b200 import dense
     g = torch.Generator(device="cuda").manual_seed(M + N)
     x = torch.relu(torch.randn(M, K, device="cuda", generator=g))
@@ -40,31 +40,27 @@ def test_pair_and_single_cta_agree_in_both_modes(M, N, K):
     b = torch.randn(N, device="cuda", generator=g) * 0.1
     ref = x.double() @ w.double().T + b.double()
     outs = {}
-    try:
-        for cl in (2, 1):
-            dense.set_cluster(cl)
-            xs, ws = dense.split(x), dense.split(w)
-            o0 = torch.empty(M, N, device="cuda")
-            dense.igemm2(xs.view(2, 1, 1, M, K), 1, 1, M, K, ws, N, 1, bias=b, out_f32=o0)
-            xt, wt = dense.tri_from_f32(x), dense.tri_from_f32(w, weight=True)
-            o1 = torch.empty(M, N, device="cuda")
-            dense.igemm2(xt.view(1, 1, M, K), 1, 1, M, K, wt, N, 1, bias=b, out_f32=o1)
-            outs[cl] = (o0, o1)
-    finally:
-        dense.set_cluster(2)
+    for rep in (0, 1):
+        xs, ws = dense.split(x), dense.split(w)
+        o0 = torch.empty(M, N, device="cuda")
+        dense.igemm2(xs.view(2, 1, 1, M, K), 1, 1, M, K, ws, N, 1, bias=b, out_f32=o0)
+        xt, wt = dense.tri_from_f32(x), dense.tri_from_f32(w, weight=True)
+        o1 = torch.empty(M, N, device="cuda")
+        dense.igemm2(xt.view(1, 1, M, K), 1, 1, M, K, wt, N, 1, bias=b, out_f32=o1)
+        outs[rep] = (o0, o1)
     torch.cuda.synchronize()
-    assert torch.equal(outs[1][0], outs[2][0]) and torch.equal(outs[1][1], outs[2][1])
-    for o in outs[2]:
+    assert torch.equal(outs[1][0], outs[0][0]) and torch.equal(outs[1][1], outs[0][1])
+    for o in outs[0]:
         assert util.rel_err(o.cpu().numpy(), ref.cpu().numpy()) < 3e-5
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout,pool", [(1, 16, 8, 64, 64, False), (3, 37, 53, 64, 64, True),
                                                  (1, 75, 125, 64, 128, False), (2, 30, 21, 128, 128, True),
                                                  (1, 16, 24, 64, 80, False)])
-def test_halo_kernel_pair_and_single_cta_agree(B, H, W, Cin, Cout, pool):
-    """Halo kernel, precision mode 1: the CTA-pair form (M = 256, each CTA holds half of every
-    tap's weights) and the single-CTA form produce the same bits in all three output planes --
-    odd tile counts (a pair with a dummy tile), ragged tiles, Cout tails, fused pooling."""
+def test_conv3x3_tri_plane_small_cout(B, H, W, Cin, Cout, pool):
+    """3x3 convolution in precision mode 1 at the low-Cout shapes of conv1_2 .. conv2_2: ragged
+    tiles, Cout tails, fused pooling; all three output planes are reproducible bit for bit and the
+    value is within 1e-4 of fp64."""
     from mnc_b200 import dense
     g = torch.Generator(device="cuda").manual_seed(H * W + Cout)
     x = torch.relu(torch.randn(B, H, W, Cin, device="cuda", generator=g))
@@ -73,16 +69,12 @@ def test_halo_kernel_pair_and_single_cta_agree(B, H, W, Cin, Cout, pool):
     xt, wt = dense.tri_from_f32(x), dense.conv_weight_to_tri(w)
     Ho, Wo = ((H + 1) // 2, (W + 1) // 2) if pool else (H, W)
     outs = {}
-    try:
-        for pair in (1, 0):
-            dense.set_halo_pair(pair)
-            o = dense.tri_alloc((B, Ho, Wo, Cout), "cuda")
-            for t in (o.h, o.l, o.c):
-                t.zero_()
-            dense.igemm2(xt, B, H, W, Cin, wt, Cout, 9, bias=b, relu=True, out=o, pool=pool, out_exp=9)
-            outs[pair] = o
-    finally:
-        dense.set_halo_pair(1)
+    for rep in (1, 0):
+        o = dense.tri_alloc((B, Ho, Wo, Cout), "cuda")
+        for t in (o.h, o.l, o.c):
+            t.zero_()
+        dense.igemm2(xt, B, H, W, Cin, wt, Cout, 9, bias=b, relu=True, out=o, pool=pool, out_exp=9)
+        outs[rep] = o
     torch.cuda.synchronize()
     for pl in ("h", "l", "c"):
         assert torch.equal(getattr(outs[1], pl), getattr(outs[0], pl)), pl
