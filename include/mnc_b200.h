@@ -94,9 +94,6 @@ int mnc_roi_warp_tri(const float* feat_nhwc, int C, int H, int W, const float* r
                      float spatial_scale, float scale, void* o14_h, void* o14_l, void* o14_c,
                      void* o7_h, void* o7_l, void* o7_c, void* stream);
 
-/* out_mode 0 epilogue: 1 (default) = stage tiles in shared memory and write them with TMA bulk
- * tensor stores; 0 = per-thread 16-byte global stores. */
-int mnc_igemm_set_tma_store(int on);
 /* Same contract as mnc_igemm_tc on the fp32 SIMT pipes (exact fp32 FMA on hi+lo operands).
  * Not on the product path: it is the on-device cross-check for the tensor-core kernel. */
 int mnc_igemm_simt(const void* a_hi, const void* a_lo, int batch, int H, int W, int Cin,
@@ -237,19 +234,6 @@ int mnc_detect_tail(const float* rois, const float* rois_ext, const float* mask,
  */
 int mnc_roi_warp_nchw(const float* feat, int C, int H, int W, const float* rois, int R,
                       int pooled_h, int pooled_w, float spatial_scale, float* out, void* stream);
-/* ROIWarping 28x28 / 14x14 kernel choice (all bit-identical):
- * 2 (default) = row walk (a warp per output plane keeps the two live feature rows in registers:
- * ~1.5 loads per output); 1 = RoI window staged in shared memory (28x28 only; 4-byte cp.async,
- * channel pairs interleaved, pairwise un-fused fp32 arithmetic); 0 = per-tap gathers through L1 (round-1
- * kernel; other pooled sizes always use it).  Returns the previous value. */
-int mnc_roi_warp_set_stage(int on);
-/* Launch shape of the row-walk kernel: threads per CTA (multiple of 32, <= 256) and channels per
- * CTA (default 128 / 32: every warp of the CTA owns planes). */
-int mnc_roi_warp_set_walk_shape(int threads, int channels_per_cta);
-int mnc_roi_warp_set_walk_planes14(int planes);   /* 14x14 row walk: planes per lane, 4 (default) or 8 */
-/* Fused engine form (mnc_roi_warp_split / mnc_roi_warp_tri): 0 (default) = per-cell gathers,
- * 1 = row walk (bit-identical outputs, 2.5x fewer loads, no faster).  Returns the previous value. */
-int mnc_roi_warp_set_rows(int on);
 int mnc_mask_resize_nchw(const float* in, int N, int C, int in_h, int in_w, int out_h, int out_w,
                          float* out, void* stream);
 int mnc_mask_pool_nchw(const float* feat, const float* mask, int N, int C, int H, int W,
@@ -259,11 +243,6 @@ int mnc_mask_pool_nchw(const float* feat, const float* mask, int N, int C, int H
 int mnc_roi_warp_split(const float* feat_nhwc /* fp32 [B][H][W][C] */, int C, int H, int W,
                        const float* rois, int R, int sub, float spatial_scale, void* o14_hi,
                        void* o14_lo, void* o7_hi, void* o7_lo, void* stream);
-/* Kernel choice for mnc_roi_warp_split: 0 (default) = one gather of 4 taps per sample, 1 =
- * column-walking kernel (separable bilinear, taps cached in registers; 2.4x fewer loads but
- * slower: serial dependence per thread).  Returns the previous setting.
- * For A/B measurement (bench.py's `micro`). */
-int mnc_roi_warp_set_walk(int on);
 int mnc_sigmoid_mask_resize(const float* logits, int stride, int R, int mask_size, int out_size,
                             float* mask_proposal, float* mask_resized, void* stream);
 int mnc_mask_pool_split(const void* f_hi, const void* f_lo, const float* mask14, int R, int C,
@@ -308,9 +287,6 @@ int mnc_mv_device(const float* boxes, const float* masks, int nb, int box_dim, i
  * previous setting.  mnc_mv_device_launches(): kernels per mnc_mv_device call (5 / 4). */
 int mnc_mv_set_two_pass(int on);
 int mnc_mv_device_launches(void);
-/* A/B knob: pixel stride of the coarse pass and CTAs per result of the coarse / border pass
- * (defaults 6, 2, 16). */
-int mnc_mv_set_shape(int stride, int chunks_coarse, int chunks_border);
 
 /* ---------------------------------------------------------------------------------------------
  * Input preparation on the device (SURVEY.md section 8f, "next" row 1): prep_im_for_blob +

@@ -888,12 +888,6 @@ static int launch_igemm(const Maps& m, const IgemmArgs& a, int max_ctas, cudaStr
 
 using namespace mnc;
 
-static int g_igemm_tma_store = 1;
-extern "C" int mnc_igemm_set_tma_store(int on) {
-  g_igemm_tma_store = on ? 1 : 0;
-  return MNC_OK;
-}
-
 // General form.  in_fmt 0: operands are split-bf16 planes (a0 = hi, a1 = lo; w0 = hi, w1 = lo);
 // in_fmt 1: tri-plane operands (a0 = fp16 value, a1 = e4m3 residual, a2 = e4m3 copy; w0 = fp16,
 // w1 = e4m3 copy, w2 = e4m3 residual -- layouts above).  out_mode 0 / 2: split-bf16 (out0 = hi,
@@ -980,7 +974,7 @@ extern "C" int mnc_igemm_tc2(int in_fmt, const void* a0, const void* a1, const v
   m.o[1] = m.a[1];
   m.o[2] = m.a[1];
   a.tma_store = 0;
-  if (out_mode == 0 && g_igemm_tma_store && out_pix_stride % 8 == 0 && out_ch_offset % 8 == 0 &&
+  if (out_mode == 0 && out_pix_stride % 8 == 0 && out_ch_offset % 8 == 0 &&
       reinterpret_cast<uintptr_t>(out0) % 16 == 0 && reinterpret_cast<uintptr_t>(out1) % 16 == 0) {
     const __nv_bfloat16* bh = static_cast<const __nv_bfloat16*>(out0) + out_ch_offset;
     const __nv_bfloat16* bl = static_cast<const __nv_bfloat16*>(out1) + out_ch_offset;

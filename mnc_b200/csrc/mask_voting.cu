@@ -628,18 +628,9 @@ extern "C" int mnc_mv_set_two_pass(int on) {
 }
 extern "C" int mnc_mv_device_launches() { return g_mv_two_pass ? 5 : 4; }
 
-// launch shape of the two passes (A/B knob): stride of the coarse pass,
+// launch shape of the two passes: stride of the coarse pass,
 // CTAs per result of the coarse / the exact border pass
-static int g_mv_stride = 6, g_mv_chunks1 = 2, g_mv_chunks2 = 16;
-extern "C" int mnc_mv_set_shape(int stride, int chunks_coarse, int chunks_border) {
-  if (stride < 1 || stride > 64 || chunks_coarse < 1 || chunks_border < 1 || chunks_coarse > 1024 ||
-      chunks_border > 1024)
-    return MNC_ERR_ARG;
-  g_mv_stride = stride;
-  g_mv_chunks1 = chunks_coarse;
-  g_mv_chunks2 = chunks_border;
-  return MNC_OK;
-}
+constexpr int g_mv_stride = 6, g_mv_chunks1 = 2, g_mv_chunks2 = 16;
 
 extern "C" int mnc_mv_device(const float* boxes, const float* masks, int nb, int box_dim,
                              int mask_size, const int* cand_inds, const float* cand_weights,

@@ -66,7 +66,6 @@ class MNCEngine:
         self.impl = impl
         self.precision = (precision or self.DEFAULT_PRECISION) if impl == "tc" else "bf16x3"
         self.tri = self.precision == "f16f8"
-        self.fuse_pool = True
         # per-tensor exponents of the tri-plane activations, measured on the first forward
         self.exp = {}
         self._calibrating = False
@@ -319,7 +318,7 @@ class MNCEngine:
             cout = couts[li]
             nxt = 1 - cur
             pool_here = name in POOL_AFTER
-            fuse = pool_here and self.impl == "tc" and self.fuse_pool
+            fuse = pool_here and self.impl == "tc"
             Ho, Wo = (_ceil_half(H), _ceil_half(W)) if pool_here else (H, W)
             # the consumer of this layer's output decides its format
             if name == "conv5_3":
