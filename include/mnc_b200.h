@@ -340,6 +340,42 @@ int mnc_roi_pool_split(const float* feat_nhwc, int C, int H, int W, const float*
 int mnc_roi_sample_split(const float* feat_nhwc, int C, int H, int W, const float* rois, int R,
                          int pooled, float spatial_scale, void* o_hi, void* o_lo, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Backward passes of the four layers, Backward_gpu contract (fp32 NCHW device blobs).  The
+ * reference's semantics are kept, quirks included (DESIGN.md "Backward semantics"); the feature
+ * and mask gradients equal the reference built with -fmad=false bit for bit.  Deterministic: no
+ * atomics, two calls on the same inputs give the same bits.  A NULL output is not computed and its
+ * memory is left untouched; R = 0 is a no-op; a RoI whose batch index lies outside [0, B)
+ * contributes nothing.  pooled_h / pooled_w outside [1, 32] -> MNC_ERR_ARG.
+ *
+ * mnc_roi_warp_backward_nchw replaces ROIWarpingLayer::Backward_gpu (roi_warping_layer.cu:379-436:
+ * ROIWarpingBackwardFeature :175-245, ROIWarpingBackwardCoordinate :306-361 and the thrust
+ * reduce_by_key :409-434).  feat (B,C,H,W) is read only for rois_diff; top_diff (R,C,ph,pw).
+ * feat_diff (B,C,H,W) is written in full; rois_diff (R,5) gets column 0 = 0 and the four
+ * coordinate gradients.  The argmax the reference stores in the forward pass is recomputed from
+ * rois.  A sample outside the map contributes 0 to rois_diff (the reference reads outside the
+ * sampled plane there).  Works in a stream-ordered allocation of R * ceil(C/64) * 32 bytes.
+ * mnc_mask_resize_backward_nchw replaces MaskResizeLayer::Backward_gpu (mask_resize_layer.cu:
+ * 135-183): top_diff (N,C,out_h,out_w) -> in_diff (N,C,in_h,in_w).
+ * mnc_mask_pool_backward_nchw replaces MaskPoolingLayer::Backward_gpu (mask_pooling_layer.cu:
+ * 43-99): feat_diff (N,C,H,W) = top_diff * mask; mask_diff (N,1,H,W) = sum over c = 0..C-1 of
+ * top_diff * feat, in that order.
+ * mnc_roi_pool_backward_nchw replaces ROIPoolingLayer::Backward_gpu (roi_pooling_layer.cu:94-184):
+ * routes top_diff (R,C,ph,pw) through argmax (int32, as mnc_roi_pool_nchw writes it) into
+ * feat_diff (B,C,H,W), written in full. */
+int mnc_roi_warp_backward_nchw(const float* feat, int B, int C, int H, int W, const float* rois,
+                               int R, int pooled_h, int pooled_w, float spatial_scale,
+                               const float* top_diff, float* feat_diff, float* rois_diff,
+                               void* stream);
+int mnc_mask_resize_backward_nchw(const float* top_diff, int N, int C, int in_h, int in_w,
+                                  int out_h, int out_w, float* in_diff, void* stream);
+int mnc_mask_pool_backward_nchw(const float* feat, const float* mask, const float* top_diff, int N,
+                                int C, int H, int W, float* feat_diff, float* mask_diff,
+                                void* stream);
+int mnc_roi_pool_backward_nchw(const float* top_diff, const int* argmax, int B, int C, int H, int W,
+                               const float* rois, int R, int pooled_h, int pooled_w,
+                               float spatial_scale, float* feat_diff, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -332,6 +332,63 @@ def roi_sample_split(feat, C, H, W, rois, pooled, out, spatial_scale=0.0625):
                                    ptr(out[0]), ptr(out[1]), cur_stream()), "mnc_roi_sample_split")
 
 
+# ----------------------------------------------------------------------------- layer backward passes
+def roi_warp_backward_nchw(feat, rois, top_diff, pooled_h, pooled_w, spatial_scale=0.0625,
+                           want_feat=True, want_rois=True):
+    """ROIWarpingLayer backward (roi_warping_layer.cu:175-436).  feat (B,C,H,W), rois (R,5),
+    top_diff (R,C,ph,pw) -> (feat_diff (B,C,H,W) or None, rois_diff (R,5) or None)."""
+    B, C, H, W = feat.shape
+    R = rois.shape[0]
+    new = torch.zeros if R == 0 else torch.empty       # R = 0: the library writes nothing
+    fd = new(feat.shape, dtype=torch.float32, device=feat.device) if want_feat else None
+    rd = new((R, 5), dtype=torch.float32, device=feat.device) if want_rois else None
+    check(lib.mnc_roi_warp_backward_nchw(ptr(feat), c_int(B), c_int(C), c_int(H), c_int(W), ptr(rois),
+                                         c_int(R), c_int(pooled_h), c_int(pooled_w),
+                                         c_float(spatial_scale), ptr(top_diff), ptr(fd), ptr(rd),
+                                         cur_stream()), "mnc_roi_warp_backward_nchw",
+          launches=int(want_feat) + 2 * int(want_rois))
+    return fd, rd
+
+
+def mask_resize_backward_nchw(top_diff, in_h, in_w):
+    """MaskResizeLayer backward (mask_resize_layer.cu:135-183): top_diff (N,C,oh,ow) -> (N,C,in_h,in_w)."""
+    N, C, oh, ow = top_diff.shape
+    out = torch.empty((N, C, in_h, in_w), dtype=torch.float32, device=top_diff.device)
+    check(lib.mnc_mask_resize_backward_nchw(ptr(top_diff), c_int(N), c_int(C), c_int(in_h), c_int(in_w),
+                                            c_int(oh), c_int(ow), ptr(out), cur_stream()),
+          "mnc_mask_resize_backward_nchw")
+    return out
+
+
+def mask_pool_backward_nchw(feat, mask, top_diff, want_feat=True, want_mask=True):
+    """MaskPoolingLayer backward (mask_pooling_layer.cu:43-99) -> (feat_diff or None, mask_diff or None)."""
+    N, C, H, W = feat.shape
+    if mask.shape != (N, 1, H, W):
+        raise ValueError("MaskPooling: mask must be (N,1,H,W) matching feat "
+                         "(mask_pooling_layer.cpp:20-29)")
+    fd = torch.empty_like(feat) if want_feat else None
+    md = torch.empty_like(mask) if want_mask else None
+    check(lib.mnc_mask_pool_backward_nchw(ptr(feat), ptr(mask), ptr(top_diff), c_int(N), c_int(C),
+                                          c_int(H), c_int(W), ptr(fd), ptr(md), cur_stream()),
+          "mnc_mask_pool_backward_nchw", launches=int(want_feat) + int(want_mask))
+    return fd, md
+
+
+def roi_pool_backward_nchw(top_diff, argmax, feat_shape, rois, pooled_h, pooled_w,
+                           spatial_scale=0.0625):
+    """ROIPoolingLayer backward (roi_pooling_layer.cu:94-184): top_diff and the int32 argmax of
+    roi_pool_nchw, both (R,C,ph,pw) -> feat_diff of feat_shape (B,C,H,W)."""
+    B, C, H, W = feat_shape
+    R = rois.shape[0]
+    new = torch.zeros if R == 0 else torch.empty
+    out = new((B, C, H, W), dtype=torch.float32, device=top_diff.device)
+    check(lib.mnc_roi_pool_backward_nchw(ptr(top_diff), ptr(argmax), c_int(B), c_int(C), c_int(H),
+                                         c_int(W), ptr(rois), c_int(R), c_int(pooled_h),
+                                         c_int(pooled_w), c_float(spatial_scale), ptr(out),
+                                         cur_stream()), "mnc_roi_pool_backward_nchw")
+    return out
+
+
 # ----------------------------------------------------------------------------- mask voting
 class VotingOverflow(RuntimeError):
     pass
