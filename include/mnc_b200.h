@@ -376,6 +376,53 @@ int mnc_roi_pool_backward_nchw(const float* top_diff, const int* argmax, int B, 
                                const float* rois, int R, int pooled_h, int pooled_w,
                                float spatial_scale, float* feat_diff, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * TRAIN phase of the cascade bridge layers, one image (IMS_PER_BATCH 1), fp32 device blobs unless
+ * stated.  The reference's numpy semantics are kept, quirks included (DESIGN.md "Training-phase
+ * bridge layers"); stream-ordered, no host synchronisation, deterministic.
+ *
+ * mnc_stage_bridge_train replaces StageBridgeLayer.forward_train (lib/pylayer/
+ * stage_bridge_layer.py:131-235).  rois [n][5], bbox_pred [n][4C], seg_cls_prob [n][C],
+ * gt_boxes [G][5] (x1,y1,x2,y2,label), gt_masks [G][mask_h][mask_w] (0/1 values), im_info [3],
+ * mask_info int32 [G][2] (height, width of each gt mask; only that crop is read, the rest counts
+ * as 0).  Host arguments: means / stds double[4] (both NULL: targets not normalised),
+ * inside_weights float[4] (cfg.TRAIN.BBOX_INSIDE_WEIGHTS), bbox_thresh (cfg.TRAIN.BBOX_THRESH),
+ * mask_size (cfg.MASK_SIZE), binarize_thresh (cfg.BINARIZE_THRESH).  Every row is kept, foreground
+ * first: with K = n + G the outputs are rois_out [K][5], labels [K], mask_targets / mask_weight
+ * [K][mask_size][mask_size], gt_mask_info [K][12], bbox_targets / bbox_inside_weights /
+ * bbox_outside_weights [K][4C], and state, int32 [2K + 2n + 1]: keep_inds [K], its inverse [K],
+ * the regression label of each RoI [n], its clip_keep flag [n], the foreground count.  n = 0 is
+ * valid; G <= 0 -> MNC_ERR_ARG.
+ *
+ * mnc_stage_bridge_train_backward replaces StageBridgeLayer.backward (:82-129): top_diff [K][5] is
+ * the diff of rois_out, state the forward's.  rois_diff [n][5] and bbox_pred_diff [n][4C] are
+ * written in full; either may be NULL (not computed, left untouched).  clip_thresh = 1 / clip_base
+ * with use_clip, 0 without.
+ *
+ * mnc_mask_layer_train replaces MaskLayer.forward_train (lib/pylayer/mask_layer.py:56-93):
+ * mask_pred [N][mask_size][mask_size], gt_masks [G][mask_h][mask_w] (0/1), gt_masks_info [N][12]
+ * as mnc_stage_bridge_train writes it -> labels [N] (region IoU >= fg_seg_thresh keeps info[3]).
+ * mnc_mask_layer_train_backward (:50-54): bottom_diff [N][mask_size^2] = top_diff where
+ * labels > 0, else 0. */
+int mnc_stage_bridge_train(const float* rois, int n, const float* bbox_pred,
+                           const float* seg_cls_prob, int num_classes, const float* gt_boxes, int G,
+                           const float* gt_masks, int mask_h, int mask_w, const float* im_info,
+                           const int* mask_info, const double* means, const double* stds,
+                           const float* inside_weights, double bbox_thresh, int mask_size,
+                           float binarize_thresh, float* rois_out, float* labels,
+                           float* mask_targets, float* mask_weight, float* gt_mask_info,
+                           float* bbox_targets, float* bbox_inside_weights,
+                           float* bbox_outside_weights, int* state, void* stream);
+int mnc_stage_bridge_train_backward(const float* top_diff, const int* state, const float* rois,
+                                    const float* bbox_pred, int n, int G, int num_classes,
+                                    float clip_thresh, float* rois_diff, float* bbox_pred_diff,
+                                    void* stream);
+int mnc_mask_layer_train(const float* mask_pred, int N, int mask_size, const float* gt_masks, int G,
+                         int mask_h, int mask_w, const float* gt_masks_info, float binarize_thresh,
+                         double fg_seg_thresh, float* labels, void* stream);
+int mnc_mask_layer_train_backward(const float* top_diff, const float* labels, int N, int mask_size,
+                                  float* bottom_diff, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,6 +7,14 @@ path.
     feat.requires_grad_(); rois.requires_grad_()
     out = autograd.roi_warp(feat, rois, 28, 28, 0.0625)
     out.sum().backward()        # feat.grad (B,C,H,W), rois.grad (R,5)
+
+The TRAIN phase of the cascade bridges (StageBridgeLayer, MaskLayer) is here too: their outputs
+that feed the next stage are differentiable, the targets they compute are not, so
+
+    rois_ext, *targets = autograd.stage_bridge_train(rois, bbox_pred, seg_cls_prob, ...)
+    autograd.roi_warp(conv5_3, rois_ext, 28, 28)
+
+carries the RoI coordinate gradient on into bbox_pred, as the 5-stage training net does.
 """
 import torch
 
@@ -96,3 +104,66 @@ def mask_pool(feat, mask):
 def roi_pool(feat, rois, pooled_h, pooled_w, spatial_scale=0.0625):
     """ROIPooling: feat (B,C,H,W), rois (R,5) -> (R,C,pooled_h,pooled_w); differentiable in feat."""
     return _RoiPool.apply(feat, rois, pooled_h, pooled_w, spatial_scale)
+
+
+class _StageBridgeTrain(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rois, bbox_pred, seg_cls_prob, gt_boxes, gt_masks, im_info, mask_info, kw,
+                clip_thresh):
+        rois, bbox_pred = _c(rois), _c(bbox_pred)
+        out = ops.stage_bridge_train(rois, bbox_pred, _c(seg_cls_prob), _c(gt_boxes), _c(gt_masks),
+                                     _c(im_info), _c(mask_info), **kw)
+        ctx.save_for_backward(rois, bbox_pred, out["state"])
+        ctx.G, ctx.clip_thresh = gt_boxes.shape[0], clip_thresh
+        targets = [out[k] for k in _BRIDGE_TARGETS]
+        ctx.mark_non_differentiable(*targets)
+        return (out["rois"], *targets)
+
+    @staticmethod
+    def backward(ctx, grad, *unused):
+        rois, bbox_pred, state = ctx.saved_tensors
+        rd, bd = ops.stage_bridge_train_backward(_c(grad), state, rois, bbox_pred, ctx.G,
+                                                 ctx.clip_thresh, want_rois=ctx.needs_input_grad[0],
+                                                 want_bbox=ctx.needs_input_grad[1])
+        return (rd, bd) + (None,) * 7
+
+
+_BRIDGE_TARGETS = ("labels", "mask_targets", "mask_weight", "gt_mask_info", "bbox_targets",
+                   "bbox_inside_weights", "bbox_outside_weights")
+
+
+class _MaskLayerTrain(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, mask_pred, gt_masks, gt_masks_info, kw):
+        N = mask_pred.shape[0]
+        labels = ops.mask_layer_train(_c(mask_pred), _c(gt_masks), _c(gt_masks_info), **kw)
+        ctx.save_for_backward(labels)
+        ctx.shape = mask_pred.shape
+        ctx.mark_non_differentiable(labels)
+        M = int(round((mask_pred.numel() // max(N, 1)) ** 0.5)) if N else 21
+        return _c(mask_pred).view(N, 1, M, M), labels.view(N, 1)
+
+    @staticmethod
+    def backward(ctx, grad, unused):
+        labels, = ctx.saved_tensors
+        return ops.mask_layer_train_backward(_c(grad), labels).view(ctx.shape), None, None, None
+
+
+def stage_bridge_train(rois, bbox_pred, seg_cls_prob, gt_boxes, gt_masks, im_info, mask_info,
+                       means=None, stds=None, inside_weights=(1.0, 1.0, 1.0, 1.0), bbox_thresh=0.5,
+                       mask_size=21, binarize_thresh=0.4, clip_thresh=0.0):
+    """StageBridgeLayer, TRAIN phase (ops.stage_bridge_train).  -> (rois_ext (K,5), labels,
+    mask_targets, mask_weight, gt_mask_info, bbox_targets, bbox_inside_weights,
+    bbox_outside_weights); rois_ext is differentiable in rois and bbox_pred (the reference's
+    backward, clip_thresh = 1 / clip_base with use_clip, else 0), the targets are not."""
+    kw = dict(means=means, stds=stds, inside_weights=inside_weights, bbox_thresh=bbox_thresh,
+              mask_size=mask_size, binarize_thresh=binarize_thresh)
+    return _StageBridgeTrain.apply(rois, bbox_pred, seg_cls_prob, gt_boxes, gt_masks, im_info,
+                                   mask_info, kw, clip_thresh)
+
+
+def mask_layer_train(mask_pred, gt_masks, gt_masks_info, binarize_thresh=0.4, fg_seg_thresh=0.5):
+    """MaskLayer, TRAIN phase (ops.mask_layer_train).  -> (mask_proposal (N,1,M,M), a reshape of
+    mask_pred differentiable in it, labels (N,1)); the gradient reaches the rows with label > 0."""
+    return _MaskLayerTrain.apply(mask_pred, gt_masks, gt_masks_info,
+                                 dict(binarize_thresh=binarize_thresh, fg_seg_thresh=fg_seg_thresh))

@@ -8,13 +8,12 @@
 // pixel and walks the instance list backwards, stopping at the last writer of that pixel -- the
 // same result without the n read-modify-write passes over the image.
 //
-// cv2.resize (OpenCV, a dependency of the reference, not part of it) is restated as in
-// preprocess.cu: fx = (dx + 0.5) * (src / dst) - 0.5 in double, floor, clamp (sx < 0 -> 0, frac 0;
-// sx >= src - 1 -> src - 1, frac 0), horizontal pass then vertical pass in fp32.
+// cv2.resize is restated in cv_resize.cuh.
 #include <cuda_runtime.h>
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "cv_resize.cuh"
 
 namespace mnc {
 
@@ -22,26 +21,6 @@ struct InstRec {
   int x1, y1, x2, y2;  // np.round(box).astype(int), clipped to the image (vis_seg.py:106-114)
   int cls;
 };
-
-__device__ __forceinline__ void cv_tap(int d, double scale, int n, int& i0, int& i1, float& a0,
-                                       float& a1) {
-  const double fd = (d + 0.5) * scale - 0.5;   // fraction in double, rounded once (see preprocess.cu)
-  int s = static_cast<int>(floor(fd));
-  float f = static_cast<float>(fd - s);
-  if (s < 0) {
-    f = 0.f;
-    s = 0;
-  }
-  if (s >= n - 1) {
-    i0 = i1 = n - 1;
-    f = 0.f;
-  } else {
-    i0 = s;
-    i1 = s + 1;
-  }
-  a0 = 1.f - f;
-  a1 = f;
-}
 
 // numpy slice [a-1 : a+1] along an axis: rows/cols {a-1, a}; empty when a == 0 (start -1 wraps to
 // the last element, past the stop).

@@ -1,5 +1,6 @@
-"""cfg constants consumed by the inference path -- reference lib/mnc_config.py (values at :16-28,
-:112-152).  Only the keys the path reads are present; the YAML merge machinery is out of scope."""
+"""cfg constants consumed by the inference path and the TRAIN phase of the cascade bridge layers --
+reference lib/mnc_config.py (values at :16-28, :63-105, :112-152).  Only the keys those read are
+present; the YAML merge machinery is out of scope."""
 import numpy as np
 
 
@@ -15,6 +16,13 @@ cfg.PIXEL_MEANS = np.array([[[102.9801, 115.9465, 122.7717]]])  # :20
 cfg.BINARIZE_THRESH = 0.4                    # :26
 cfg.MASK_SIZE = 21                           # :28
 cfg.TRAIN = _AttrDict(MAX_SIZE=1000, SCALES=(600,))
+# experiments/cfgs/VGG16/mnc_5stage.yml:6 sets True for the 5-stage net; the default is :64's
+cfg.TRAIN.BBOX_NORMALIZE_TARGETS_PRECOMPUTED = False
+cfg.TRAIN.BBOX_THRESH = 0.5                  # :65
+cfg.TRAIN.BBOX_NORMALIZE_MEANS = (0.0, 0.0, 0.0, 0.0)   # :66
+cfg.TRAIN.BBOX_NORMALIZE_STDS = (0.1, 0.1, 0.2, 0.2)    # :67
+cfg.TRAIN.BBOX_INSIDE_WEIGHTS = (1.0, 1.0, 1.0, 1.0)    # :69
+cfg.TRAIN.FG_SEG_THRESH = 0.5                # :105
 cfg.TEST = _AttrDict()
 cfg.TEST.SCALES = (600,)                     # :115
 cfg.TEST.MAX_SIZE = 1000                     # :118

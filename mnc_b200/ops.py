@@ -555,3 +555,87 @@ def binarize_masks(rboxes, masks, thresh=0.4):
                                  c_float(thresh), ptr(d_off), c_int(int(areas.max()) if n else 0),
                                  ptr(out), cur_stream()), "mnc_binarize_masks")
     return out, offsets
+
+
+# ------------------------------------------------------------ training-phase cascade bridge layers
+def _f32(t):
+    return t.contiguous().to(torch.float32)
+
+
+def stage_bridge_train(rois, bbox_pred, seg_cls_prob, gt_boxes, gt_masks, im_info, mask_info,
+                       means=None, stds=None, inside_weights=(1.0, 1.0, 1.0, 1.0), bbox_thresh=0.5,
+                       mask_size=21, binarize_thresh=0.4):
+    """StageBridgeLayer.forward_train (lib/pylayer/stage_bridge_layer.py:131-235), one image.
+    Device tensors rois (n,5), bbox_pred (n,4C), seg_cls_prob (n,C), gt_boxes (G,5), gt_masks
+    (G,Hm,Wm) 0/1, im_info (3,), mask_info (G,2).  means / stds (4 floats each, or None: targets
+    not normalised) are cfg.TRAIN.BBOX_NORMALIZE_MEANS / STDS when
+    BBOX_NORMALIZE_TARGETS_PRECOMPUTED.  -> dict of the eight tops (K = n + G rows, foreground
+    first) and `state`, the int32 buffer mnc_stage_bridge_train_backward reads."""
+    n, G = rois.shape[0], gt_boxes.shape[0]
+    C = seg_cls_prob.shape[1]
+    if bbox_pred.shape != (n, 4 * C) or gt_masks.dim() != 3 or mask_info.shape != (G, 2):
+        raise ValueError("stage_bridge_train: inconsistent shapes")
+    if (means is None) != (stds is None):
+        raise ValueError("stage_bridge_train: give both means and stds, or neither")
+    K, M, dev = n + G, mask_size, rois.device
+    e = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
+    out = {"rois": e(K, 5), "labels": e(K), "mask_targets": e(K, 1, M, M),
+           "mask_weight": e(K, 1, M, M), "gt_mask_info": e(K, 12), "bbox_targets": e(K, 4 * C),
+           "bbox_inside_weights": e(K, 4 * C), "bbox_outside_weights": e(K, 4 * C),
+           "state": torch.empty(2 * K + 2 * n + 1, dtype=torch.int32, device=dev)}
+    dbl4 = lambda v: None if v is None else (ctypes.c_double * 4)(*[float(x) for x in v])
+    gm = _f32(gt_masks)
+    check(lib.mnc_stage_bridge_train(
+        ptr(_f32(rois)), c_int(n), ptr(_f32(bbox_pred)), ptr(_f32(seg_cls_prob)), c_int(C),
+        ptr(_f32(gt_boxes)), c_int(G), ptr(gm), c_int(gm.shape[1]), c_int(gm.shape[2]),
+        ptr(_f32(im_info)), ptr(mask_info.contiguous().to(torch.int32)), dbl4(means), dbl4(stds),
+        (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), ctypes.c_double(bbox_thresh),
+        c_int(M), c_float(binarize_thresh), *[ptr(out[k]) for k in (
+            "rois", "labels", "mask_targets", "mask_weight", "gt_mask_info", "bbox_targets",
+            "bbox_inside_weights", "bbox_outside_weights", "state")], cur_stream()),
+        "mnc_stage_bridge_train", launches=2)
+    return out
+
+
+def stage_bridge_train_backward(top_diff, state, rois, bbox_pred, G, clip_thresh=0.0,
+                                want_rois=True, want_bbox=True):
+    """StageBridgeLayer.backward (stage_bridge_layer.py:82-129).  top_diff (K,5) is the diff of the
+    `rois` top; clip_thresh = 1 / clip_base with use_clip, else 0.
+    -> (rois_diff (n,5) or None, bbox_pred_diff (n,4C) or None)."""
+    n = rois.shape[0]
+    C4 = bbox_pred.shape[1]
+    dev = rois.device
+    new = torch.zeros if n == 0 else torch.empty
+    rd = new((n, 5), dtype=torch.float32, device=dev) if want_rois else None
+    bd = new((n, C4), dtype=torch.float32, device=dev) if want_bbox else None
+    check(lib.mnc_stage_bridge_train_backward(
+        ptr(_f32(top_diff)), ptr(state), ptr(_f32(rois)), ptr(_f32(bbox_pred)), c_int(n), c_int(G),
+        c_int(C4 // 4), c_float(clip_thresh), ptr(rd), ptr(bd), cur_stream()),
+        "mnc_stage_bridge_train_backward", launches=int(n > 0 and (want_rois or want_bbox)))
+    return rd, bd
+
+
+def mask_layer_train(mask_pred, gt_masks, gt_masks_info, binarize_thresh=0.4, fg_seg_thresh=0.5):
+    """MaskLayer.forward_train (lib/pylayer/mask_layer.py:56-93): mask_pred (N,M*M) or
+    (N,1,M,M), gt_masks (G,Hm,Wm) 0/1, gt_masks_info (N,12) as stage_bridge_train writes it
+    -> labels (N,) float32."""
+    N = mask_pred.shape[0]
+    M = int(round((mask_pred.numel() // max(N, 1)) ** 0.5)) if N else 21
+    gm = _f32(gt_masks)
+    labels = torch.empty((N,), dtype=torch.float32, device=mask_pred.device)
+    check(lib.mnc_mask_layer_train(ptr(_f32(mask_pred)), c_int(N), c_int(M), ptr(gm), c_int(gm.shape[0]),
+                                   c_int(gm.shape[1]), c_int(gm.shape[2]), ptr(_f32(gt_masks_info)),
+                                   c_float(binarize_thresh), ctypes.c_double(fg_seg_thresh),
+                                   ptr(labels), cur_stream()), "mnc_mask_layer_train")
+    return labels
+
+
+def mask_layer_train_backward(top_diff, labels):
+    """MaskLayer.backward (mask_layer.py:50-54): rows with label > 0 copy top_diff, others 0.
+    top_diff (N,1,M,M) -> (N,M*M)."""
+    N = top_diff.shape[0]
+    M = top_diff.shape[-1]
+    out = torch.empty((N, M * M), dtype=torch.float32, device=top_diff.device)
+    check(lib.mnc_mask_layer_train_backward(ptr(_f32(top_diff)), ptr(_f32(labels)), c_int(N), c_int(M),
+                                            ptr(out), cur_stream()), "mnc_mask_layer_train_backward")
+    return out
