@@ -79,7 +79,9 @@ int mnc_igemm_tc2(int in_fmt, const void* a0, const void* a1, const void* a2, in
 int mnc_f32_to_tri(const float* in, long long n, float scale, void* h, void* l, void* c,
                    unsigned int* amax, void* stream);
 int mnc_tri_to_f32(const void* h, const void* l, long long n, float inv_scale, float* out, void* stream);
-/* mnc_splitk_reduce with a tri-plane result. */
+/* mnc_splitk_reduce with a tri-plane result.  This entry point, mnc_mask_pool_tri and
+ * mnc_roi_warp_tri move four elements at a time: every fp16 plane (h) must be 8-byte aligned and
+ * every e4m3 plane (l, c) 4-byte aligned, or they return MNC_ERR_ARG. */
 int mnc_splitk_reduce_tri(const float* partial, int splits, long long split_stride, long long rows,
                           int cols, const float* bias, int relu, float scale, void* h, void* l,
                           void* c, long long out_row_stride, int out_ch_offset, unsigned int* amax,

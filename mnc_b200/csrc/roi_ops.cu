@@ -753,7 +753,8 @@ extern "C" int mnc_roi_warp_tri(const float* feat_nhwc, int C, int H, int W, con
                                 void* o14_l, void* o14_c, void* o7_h, void* o7_l, void* o7_c,
                                 void* stream) {
   if (R <= 0) return MNC_OK;
-  if (C % 4 != 0 || (sub != 1 && sub != 2) || (reinterpret_cast<uintptr_t>(feat_nhwc) & 15))
+  if (C % 4 != 0 || (sub != 1 && sub != 2) || (reinterpret_cast<uintptr_t>(feat_nhwc) & 15) ||
+      !tri_planes_aligned(o14_h, o14_l, o14_c) || !tri_planes_aligned(o7_h, o7_l, o7_c))
     return MNC_ERR_ARG;
   auto s = static_cast<cudaStream_t>(stream);
   RoiOut o;

@@ -49,4 +49,11 @@ __device__ __forceinline__ float4 ld_tri4(const __half* h, const uint8_t* l, lon
   return make_float4(a.x, a.y, b.x, b.y);
 }
 
+// Host-side argument check of the entry points that use st_tri4 / ld_tri4: four elements move at a
+// time, 8 bytes of the fp16 plane and 4 bytes of each e4m3 plane (c may be null: not accessed).
+inline bool tri_planes_aligned(const void* h, const void* l, const void* c) {
+  return reinterpret_cast<uintptr_t>(h) % 8 == 0 && reinterpret_cast<uintptr_t>(l) % 4 == 0 &&
+         (c == nullptr || reinterpret_cast<uintptr_t>(c) % 4 == 0);
+}
+
 }  // namespace mnc

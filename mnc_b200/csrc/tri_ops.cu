@@ -146,7 +146,7 @@ extern "C" int mnc_splitk_reduce_tri(const float* partial, int splits, long long
   if (rows <= 0 || cols <= 0) return MNC_OK;
   if (cols % 4 != 0 || split_stride % 4 != 0 || out_row_stride % 4 != 0 || out_ch_offset % 4 != 0 ||
       reinterpret_cast<uintptr_t>(partial) % 16 != 0 ||
-      (bias != nullptr && reinterpret_cast<uintptr_t>(bias) % 16 != 0))
+      (bias != nullptr && reinterpret_cast<uintptr_t>(bias) % 16 != 0) || !tri_planes_aligned(h, l, c))
     return MNC_ERR_ARG;
   splitk_reduce_tri_kernel<<<tri_grid(rows * (cols / 4), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       partial, splits, split_stride, rows, cols, bias, relu, scale, static_cast<__half*>(h),
@@ -157,7 +157,8 @@ extern "C" int mnc_splitk_reduce_tri(const float* partial, int splits, long long
 extern "C" int mnc_mask_pool_tri(const void* f_h, const void* f_l, const float* mask14, int R, int C,
                                  void* o_h, void* o_l, void* o_c, void* stream) {
   if (R <= 0) return MNC_OK;
-  if (C % 4 != 0) return MNC_ERR_ARG;
+  if (C % 4 != 0 || !tri_planes_aligned(f_h, f_l, nullptr) || !tri_planes_aligned(o_h, o_l, o_c))
+    return MNC_ERR_ARG;
   dim3 grid(R, 7);
   mask_pool_tri_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __half*>(f_h), static_cast<const uint8_t*>(f_l), mask14, C,
