@@ -425,6 +425,77 @@ int mnc_mask_layer_train(const float* mask_pred, int N, int mask_size, const flo
 int mnc_mask_layer_train_backward(const float* top_diff, const float* labels, int N, int mask_size,
                                   float* bottom_diff, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * TRAIN phase of the RPN-stage layers (ProposalLayer, ProposalTargetLayer, AnchorTargetLayer), one
+ * image, fp32 device blobs unless stated; stream-ordered, no host synchronisation, deterministic
+ * (DESIGN.md "RPN-stage training layers").  The reference's npr.choice(cands, size) is replaced by a
+ * choice the caller's random keys (uint32) decide: the `size` candidates with the smallest
+ * (key, index) pairs.
+ *
+ * mnc_proposal_train_state completes ProposalLayer.forward's TRAIN tops (lib/pylayer/
+ * proposal_layer.py:52-175) after the TEST chain (mnc_rpn_decode .. mnc_write_rois): order is the
+ * score order of the decoded anchors, keep / num_keep the NMS result, R the number of rows written
+ * (RPN_POST_NMS_TOP_N).  rpn_bbox_pred (1,4A,H,W), im_info [3].  Writes proposal_index [R] (the
+ * anchor index in (h, w, a) order, -1 past num_keep) and state int32 [R][2] (anchor index, the
+ * product of the two clip_boxes keep tests) for mnc_proposal_backward (:177-230), which zeroes
+ * bbox_pred_diff (1,4A,H,W) and writes the rows of top_diff [R][5] that are not all zero;
+ * clip_thresh = 1 / clip_base with use_clip, else 0.  bbox_pred_diff NULL: nothing is done.
+ *
+ * mnc_proposal_target replaces ProposalTargetLayer.forward (proposal_target_layer.py:62-107,
+ * :118-216): rpn_rois [n][5], rpn_rois_index [n] (MIX_INDEX; NULL when n = 0), n_valid (device
+ * int: only rows < *n_valid are RoIs, the rest padding, e.g. mnc_write_rois' count; NULL: all n),
+ * gt_boxes [G][5], gt_masks [G][mask_h][mask_w] (0/1), mask_info int32 [G][2], im_info [3], keys uint32
+ * [n_fg_cats + n_bg_cats][n + G] (one row per sampling category).  Host config: BATCH_SIZE, the
+ * FG / BG FRACTION and THRESH_LO / HI lists (at most 4 each, fractions summing to <= 1 + 1e-9), means /
+ * stds double[4] (both NULL: not normalised), inside_weights float[4], mask_size, binarize_thresh,
+ * num_classes.  Outputs are written at k_max = mnc_proposal_target_capacity(...) rows: rois [k_max][5],
+ * labels [k_max], bbox_targets / inside / outside weights [k_max][4C], mask_targets / mask_weight
+ * [k_max][mask_size^2], gt_masks_info [k_max][12], fg_inds / bg_inds [k_max] (MIX_INDEX lists, -1
+ * padded); counts int32 [4] = K, #fg_inds, #bg_inds, #foreground rows.  Rows >= K: label -1, zero
+ * RoI, targets, weights and masks, gt_masks_info -1.  state int32
+ * [mnc_proposal_target_state_ints(n, G, k_max)] feeds mnc_proposal_target_backward (:109-115),
+ * which writes rpn_rois_diff [n][5] in full (NULL: nothing is done); bp_all 0 copies only the fg rows.
+ * G <= 0 -> MNC_ERR_ARG (the reference's argmax over no gt boxes raises).
+ *
+ * mnc_anchor_target replaces AnchorTargetLayer.forward (anchor_target_layer.py:51-209): an H x W map
+ * at feat_stride, gt_boxes [G][5], im_info [3], keys uint32 [H*W*A] in (h, w, a) order, fg_inds /
+ * bg_inds with their counts at mix_counts[1] / [2] (mnc_proposal_target's counts; all three NULL
+ * without MIX_INDEX), mix_cap their capacity.  Host config: RPN_NEGATIVE / POSITIVE_OVERLAP,
+ * RPN_CLOBBER_POSITIVES, RPN_FG_FRACTION (in [0, 1]), RPN_BATCHSIZE, RPN_POSITIVE_WEIGHT,
+ * RPN_BBOX_INSIDE_WEIGHTS.  workspace of mnc_anchor_target_workspace_bytes(H, W, G) bytes.  Writes
+ * labels (1,1,A*H,W) and bbox_targets / bbox_inside_weights / bbox_outside_weights (1,4A,H,W).
+ * G <= 0 -> MNC_ERR_ARG. */
+int mnc_proposal_train_state(const int* order, const int* keep, const int* num_keep, int R,
+                             const float* rpn_bbox_pred, int H, int W, int feat_stride,
+                             const float* im_info, float* proposal_index, int* state, void* stream);
+int mnc_proposal_backward(const float* top_diff, int R, const int* state,
+                          const float* rpn_bbox_pred, int H, int W, float clip_thresh,
+                          float* bbox_pred_diff, void* stream);
+int mnc_proposal_target_capacity(int batch_size, int n_fg_cats, int n_bg_cats);
+long long mnc_proposal_target_state_ints(int n, int G, int k_max);
+int mnc_proposal_target(
+    const float* rpn_rois, int n, const float* rpn_rois_index, const int* n_valid,
+    const float* gt_boxes, int G, const float* gt_masks, int mask_h, int mask_w,
+    const int* mask_info, const float* im_info, const unsigned* keys, int batch_size, int n_fg_cats, const double* fg_fraction,
+    const double* fg_thresh_lo, const double* fg_thresh_hi, int n_bg_cats,
+    const double* bg_fraction, const double* bg_thresh_lo, const double* bg_thresh_hi,
+    const double* means, const double* stds, const float* inside_weights, int mask_size,
+    float binarize_thresh, int num_classes, int k_max, float* rois, float* labels,
+    float* bbox_targets, float* bbox_inside_weights, float* bbox_outside_weights,
+    float* mask_targets, float* mask_weight, float* gt_masks_info, float* fg_inds,
+    float* bg_inds, int* counts, int* state, void* stream);
+int mnc_proposal_target_backward(const float* top_diff, const int* state, int n, int G,
+                                 int bp_all, float* rpn_rois_diff, void* stream);
+long long mnc_anchor_target_workspace_bytes(int H, int W, int G);
+int mnc_anchor_target(int H, int W, int feat_stride, int allowed_border, const float* gt_boxes,
+                      int G, const float* im_info, const unsigned* keys, const float* fg_inds,
+                      const float* bg_inds, const int* mix_counts, int mix_cap,
+                      double negative_overlap, double positive_overlap, int clobber_positives,
+                      double fg_fraction, int batch_size, double positive_weight,
+                      const float* inside_weights, void* workspace, float* labels,
+                      float* bbox_targets, float* bbox_inside_weights,
+                      float* bbox_outside_weights, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,8 +8,9 @@ path.
     out = autograd.roi_warp(feat, rois, 28, 28, 0.0625)
     out.sum().backward()        # feat.grad (B,C,H,W), rois.grad (R,5)
 
-The TRAIN phase of the cascade bridges (StageBridgeLayer, MaskLayer) is here too: their outputs
-that feed the next stage are differentiable, the targets they compute are not, so
+The TRAIN phase of the cascade bridges (StageBridgeLayer, MaskLayer) and of the RPN-stage layers
+(ProposalLayer, ProposalTargetLayer, AnchorTargetLayer) is here too: their outputs that feed the
+next stage are differentiable, the targets they compute are not, so
 
     rois_ext, *targets = autograd.stage_bridge_train(rois, bbox_pred, seg_cls_prob, ...)
     autograd.roi_warp(conv5_3, rois_ext, 28, 28)
@@ -167,3 +168,87 @@ def mask_layer_train(mask_pred, gt_masks, gt_masks_info, binarize_thresh=0.4, fg
     mask_pred differentiable in it, labels (N,1)); the gradient reaches the rows with label > 0."""
     return _MaskLayerTrain.apply(mask_pred, gt_masks, gt_masks_info,
                                  dict(binarize_thresh=binarize_thresh, fg_seg_thresh=fg_seg_thresh))
+
+
+# --------------------------------------------------------------------- RPN-stage training layers
+class _ProposalTrain(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rpn_cls_prob, rpn_bbox_pred, im_info, H, W, kw, clip_thresh):
+        bbox = _c(rpn_bbox_pred)
+        rois, index, count, state = ops.proposal_train(_c(rpn_cls_prob), bbox, _c(im_info), H, W, **kw)
+        ctx.save_for_backward(bbox, state)
+        ctx.clip_thresh = clip_thresh
+        ctx.mark_non_differentiable(index, count)
+        return rois, index, count
+
+    @staticmethod
+    def backward(ctx, grad, *unused):
+        bbox, state = ctx.saved_tensors
+        if not ctx.needs_input_grad[1]:
+            return (None,) * 7
+        return None, ops.proposal_backward(_c(grad), state, bbox, ctx.clip_thresh), None, None, None, None, None
+
+
+class _ProposalTarget(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_info, keys, kw,
+                bp_all):
+        out = ops.proposal_target(_c(rpn_rois), _c(rpn_rois_index), _c(gt_boxes), _c(gt_masks),
+                                  _c(mask_info), _c(im_info), _c(keys), **kw)
+        ctx.save_for_backward(out["state"])
+        ctx.nG = (rpn_rois.shape[0], gt_boxes.shape[0])
+        ctx.bp_all = bp_all
+        targets = [out[k] for k in PROPOSAL_TARGET_TOPS[1:]] + [out["counts"]]
+        ctx.mark_non_differentiable(*targets)
+        return (out["rois"], *targets)
+
+    @staticmethod
+    def backward(ctx, grad, *unused):
+        state, = ctx.saved_tensors
+        rd = ops.proposal_target_backward(_c(grad), state, *ctx.nG, ctx.bp_all) \
+            if ctx.needs_input_grad[0] else None
+        return (rd,) + (None,) * 8
+
+
+PROPOSAL_TARGET_TOPS = ("rois", "labels", "bbox_targets", "bbox_inside_weights",
+                        "bbox_outside_weights", "mask_targets", "mask_weight", "gt_masks_info",
+                        "fg_inds", "bg_inds")
+
+
+def proposal_train(rpn_cls_prob, rpn_bbox_pred, im_info, pre_nms_top_n=12000, post_nms_top_n=300,
+                   nms_thresh=0.7, min_size=16.0, clip_thresh=0.0):
+    """ProposalLayer, TRAIN phase (ops.proposal_train).  rpn_cls_prob (1,2A,H,W), rpn_bbox_pred
+    (1,4A,H,W).  -> (rois (R,5), proposal_index (R,), count (1,)); rois is differentiable in
+    rpn_bbox_pred with the reference's backward (clip_thresh = 1 / clip_base with use_clip, else
+    0).  R = post_nms_top_n; rows past count are zero RoIs with index -1: pass count on to
+    proposal_target, which then ignores them (no synchronisation).  Defaults: cfg.TRAIN with mnc_5stage.yml's RPN_POST_NMS_TOP_N."""
+    H, W = rpn_bbox_pred.shape[-2:]
+    kw = dict(pre_nms_top_n=pre_nms_top_n, post_nms_top_n=post_nms_top_n, nms_thresh=nms_thresh,
+              min_size=min_size)
+    return _ProposalTrain.apply(rpn_cls_prob, rpn_bbox_pred, im_info, H, W, kw, clip_thresh)
+
+
+def proposal_target(rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_info, keys=None,
+                    bp_all=True, count=None, **kw):
+    """ProposalTargetLayer (ops.proposal_target; keyword config as there).  keys None: drawn with
+    ops.sample_keys (torch's generator on the device).  count: proposal_train's device count, the
+    rows of rpn_rois that are RoIs (None: all).  -> (rois, labels, bbox_targets,
+    bbox_inside_weights, bbox_outside_weights, mask_targets, mask_weight, gt_masks_info, fg_inds,
+    bg_inds, counts), padded to the capacity; rois is differentiable in rpn_rois (the rows of
+    keep_inds, or of the fg rows with bp_all off), the rest is not."""
+    if keys is None:
+        ncat = len(kw.get("fg_fraction", (0.3,))) + len(kw.get("bg_fraction", (0.85, 0.15)))
+        keys = ops.sample_keys(ncat, rpn_rois.shape[0] + gt_boxes.shape[0], device=rpn_rois.device)
+    return _ProposalTarget.apply(rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_info,
+                                 keys, dict(kw, n_valid=count), bp_all)
+
+
+def anchor_target(H, W, gt_boxes, im_info, fg_inds=None, bg_inds=None, counts=None, keys=None,
+                  **kw):
+    """AnchorTargetLayer (ops.anchor_target; not differentiable).  keys None: drawn with
+    ops.sample_keys."""
+    if keys is None:
+        keys = ops.sample_keys(H * W * 9, device=gt_boxes.device)
+    with torch.no_grad():
+        return ops.anchor_target(H, W, gt_boxes.detach(), im_info.detach(), keys, fg_inds, bg_inds,
+                                 counts, **kw)

@@ -12,6 +12,7 @@
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "bbox_decode.cuh"
 
 namespace mnc {
 
@@ -51,19 +52,12 @@ static void generate_anchors_host(double out[9][4]) {
 
 __device__ __forceinline__ float clipf(float v, float hi) { return fmaxf(fminf(v, hi), 0.f); }
 
-// bbox_transform_inv for one box / one delta quadruple (bbox_transform.py:72-97), then
-// clip_boxes (:112-118).  All fp32, one rounding per numpy operation.
+// bbox_transform_inv (bbox_decode.cuh), then clip_boxes (bbox_transform.py:112-118).
 __device__ __forceinline__ void decode_clip(float x1, float y1, float x2, float y2, float dx,
                                             float dy, float dw, float dh, float im_h, float im_w,
                                             float out[4]) {
-  const float widths = __fadd_rn(__fsub_rn(x2, x1), 1.0f);
-  const float heights = __fadd_rn(__fsub_rn(y2, y1), 1.0f);
-  const float ctr_x = __fadd_rn(x1, __fmul_rn(0.5f, widths));
-  const float ctr_y = __fadd_rn(y1, __fmul_rn(0.5f, heights));
-  const float pred_ctr_x = __fadd_rn(__fmul_rn(dx, widths), ctr_x);
-  const float pred_ctr_y = __fadd_rn(__fmul_rn(dy, heights), ctr_y);
-  const float pred_w = __fmul_rn(expf(dw), widths);
-  const float pred_h = __fmul_rn(expf(dh), heights);
+  float pred_ctr_x, pred_ctr_y, pred_w, pred_h;
+  decode_center(x1, y1, x2, y2, dx, dy, dw, dh, pred_ctr_x, pred_ctr_y, pred_w, pred_h);
   const float wmax = __fsub_rn(im_w, 1.0f), hmax = __fsub_rn(im_h, 1.0f);
   out[0] = clipf(__fsub_rn(pred_ctr_x, __fmul_rn(0.5f, pred_w)), wmax);
   out[1] = clipf(__fsub_rn(pred_ctr_y, __fmul_rn(0.5f, pred_h)), hmax);

@@ -639,3 +639,144 @@ def mask_layer_train_backward(top_diff, labels):
     check(lib.mnc_mask_layer_train_backward(ptr(_f32(top_diff)), ptr(_f32(labels)), c_int(N), c_int(M),
                                             ptr(out), cur_stream()), "mnc_mask_layer_train_backward")
     return out
+
+
+# ------------------------------------------------------------------ training-phase RPN-stage layers
+lib.mnc_proposal_target_state_ints.restype = ctypes.c_longlong
+lib.mnc_anchor_target_workspace_bytes.restype = ctypes.c_longlong
+
+
+def sample_keys(*shape, device):
+    """Random uint32 sampling keys (as int32) from torch's generator on `device`: the chosen subset
+    of a category is its candidates with the smallest (key, index) pairs (include/mnc_b200.h)."""
+    return torch.randint(-2 ** 31, 2 ** 31, shape, dtype=torch.int32, device=device)
+
+
+def proposal_train(cls, bbox, im_info, H, W, pre_nms_top_n=12000, post_nms_top_n=300,
+                   nms_thresh=0.7, min_size=16.0, feat_stride=16):
+    """ProposalLayer.forward, TRAIN phase (lib/pylayer/proposal_layer.py:52-175), one image: the
+    TEST chain, then the proposal_index top and the backward's state.  cls (1,2A,H,W) scores,
+    bbox (1,4A,H,W).  -> (rois (R,5), proposal_index (R,), count int32 (1,), state int32 (R,2));
+    rows past count are zero RoIs with index -1."""
+    cls, bbox, im_info = _f32(cls), _f32(bbox), _f32(im_info).view(1, 3)
+    rois, counts, mid = proposals_from_rpn(cls, bbox, im_info, 1, H, W, "nchw", apply_softmax=False,
+                                           pre_nms_top_n=pre_nms_top_n, post_nms_top_n=post_nms_top_n,
+                                           nms_thresh=nms_thresh, min_size=min_size,
+                                           batch_index_mode=False, return_intermediate=True)
+    R = rois.shape[1]
+    index = torch.empty((R,), dtype=torch.float32, device=cls.device)
+    state = _i32(R, 2, device=cls.device)
+    check(lib.mnc_proposal_train_state(ptr(mid["order"]), ptr(mid["keep"]), ptr(mid["num"]), c_int(R),
+                                       ptr(bbox), c_int(H), c_int(W), c_int(feat_stride), ptr(im_info),
+                                       ptr(index), ptr(state), cur_stream()),
+          "mnc_proposal_train_state", launches=int(R > 0))
+    return rois[0], index, counts, state
+
+
+def proposal_backward(top_diff, state, bbox, clip_thresh=0.0):
+    """ProposalLayer.backward (proposal_layer.py:177-230): top_diff (R,5) of the rois top, bbox
+    (1,4A,H,W) the rpn_bbox_pred data -> its diff (1,4A,H,W)."""
+    bbox = _f32(bbox)
+    H, W = bbox.shape[-2:]
+    out = torch.empty_like(bbox)
+    R = state.shape[0]
+    check(lib.mnc_proposal_backward(ptr(_f32(top_diff)), c_int(R), ptr(state), ptr(bbox), c_int(H),
+                                    c_int(W), c_float(clip_thresh), ptr(out), cur_stream()),
+          "mnc_proposal_backward", launches=1 + int(R > 0))
+    return out
+
+
+def proposal_target_capacity(batch_size, fg_fraction, bg_fraction):
+    return int(lib.mnc_proposal_target_capacity(c_int(batch_size), c_int(len(fg_fraction)),
+                                                c_int(len(bg_fraction))))
+
+
+def proposal_target(rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_info, keys,
+                    batch_size=64, fg_fraction=(0.3,), fg_thresh_lo=(0.5,), fg_thresh_hi=(1.0,),
+                    bg_fraction=(0.85, 0.15), bg_thresh_lo=(0.1, 0.0), bg_thresh_hi=(0.5, 0.1),
+                    means=None, stds=None, inside_weights=(1.0, 1.0, 1.0, 1.0), mask_size=21,
+                    binarize_thresh=0.4, num_classes=21, n_valid=None):
+    """ProposalTargetLayer.forward (lib/pylayer/proposal_target_layer.py:62-107,118-216), one image.
+    rpn_rois (n,5), rpn_rois_index (n,) or (1,n) (MIX_INDEX), gt_boxes (G,5), gt_masks (G,Hm,Wm)
+    0/1, mask_info (G,2), im_info (3,), keys int32 (len(fg_fraction) + len(bg_fraction), n + G).
+    Config defaults are cfg.TRAIN's (lib/mnc_config.py:36-69); means / stds None: targets not
+    normalised.  n_valid: int32 device count (proposal_train's `count`) -- rows of rpn_rois past it
+    are padding and take no part -- or None: all n rows are RoIs.  -> dict of the tops at Kmax = proposal_target_capacity(...) rows, `counts` int32
+    (4,) = K, #fg_inds, #bg_inds, #fg rows, and `state` for proposal_target_backward."""
+    n, G = rpn_rois.shape[0], gt_boxes.shape[0]
+    ncat = len(fg_fraction) + len(bg_fraction)
+    if keys.shape != (ncat, n + G) or mask_info.shape != (G, 2) or gt_masks.dim() != 3:
+        raise ValueError("proposal_target: inconsistent shapes")
+    if (means is None) != (stds is None):
+        raise ValueError("proposal_target: give both means and stds, or neither")
+    dev = rpn_rois.device
+    Kmax = proposal_target_capacity(batch_size, fg_fraction, bg_fraction)
+    M, C = mask_size, num_classes
+    e = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
+    out = {"rois": e(Kmax, 5), "labels": e(Kmax), "bbox_targets": e(Kmax, 4 * C),
+           "bbox_inside_weights": e(Kmax, 4 * C), "bbox_outside_weights": e(Kmax, 4 * C),
+           "mask_targets": e(Kmax, 1, M, M), "mask_weight": e(Kmax, 1, M, M),
+           "gt_masks_info": e(Kmax, 12), "fg_inds": e(Kmax), "bg_inds": e(Kmax),
+           "counts": _i32(4, device=dev),
+           "state": _i32(int(lib.mnc_proposal_target_state_ints(c_int(n), c_int(G), c_int(Kmax))),
+                         device=dev)}
+    dbl = lambda v: None if v is None else (c_double * len(v))(*[float(x) for x in v])
+    gm = _f32(gt_masks)
+    idx = _f32(rpn_rois_index).reshape(-1) if n else None
+    check(lib.mnc_proposal_target(
+        ptr(_f32(rpn_rois)), c_int(n), ptr(idx),
+        ptr(None if n_valid is None else n_valid.contiguous().to(torch.int32)), ptr(_f32(gt_boxes)),
+        c_int(G), ptr(gm),
+        c_int(gm.shape[1]), c_int(gm.shape[2]), ptr(mask_info.contiguous().to(torch.int32)),
+        ptr(_f32(im_info)), ptr(keys.contiguous().to(torch.int32)), c_int(batch_size),
+        c_int(len(fg_fraction)), dbl(fg_fraction), dbl(fg_thresh_lo), dbl(fg_thresh_hi),
+        c_int(len(bg_fraction)), dbl(bg_fraction), dbl(bg_thresh_lo), dbl(bg_thresh_hi),
+        dbl(means), dbl(stds), (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), c_int(M),
+        c_float(binarize_thresh), c_int(C), c_int(Kmax), *[ptr(out[k]) for k in (
+            "rois", "labels", "bbox_targets", "bbox_inside_weights", "bbox_outside_weights",
+            "mask_targets", "mask_weight", "gt_masks_info", "fg_inds", "bg_inds", "counts",
+            "state")], cur_stream()), "mnc_proposal_target", launches=2)
+    return out
+
+
+def proposal_target_backward(top_diff, state, n, G, bp_all=True):
+    """ProposalTargetLayer.backward (proposal_target_layer.py:109-115): top_diff (Kmax,5) of the
+    rois top -> rpn_rois diff (n,5); rows >= K of top_diff are never read."""
+    dev = state.device
+    out = (torch.zeros if n == 0 else torch.empty)((n, 5), dtype=torch.float32, device=dev)
+    check(lib.mnc_proposal_target_backward(ptr(_f32(top_diff)), ptr(state), c_int(n), c_int(G),
+                                           c_int(int(bool(bp_all))), ptr(out), cur_stream()),
+          "mnc_proposal_target_backward", launches=int(n > 0))
+    return out
+
+
+def anchor_target(H, W, gt_boxes, im_info, keys, fg_inds=None, bg_inds=None, counts=None,
+                  feat_stride=16, allowed_border=0, negative_overlap=0.3, positive_overlap=0.7,
+                  clobber_positives=False, fg_fraction=0.5, batch_size=256, positive_weight=-1.0,
+                  inside_weights=(1.0, 1.0, 1.0, 1.0)):
+    """AnchorTargetLayer.forward (lib/pylayer/anchor_target_layer.py:51-209), one image.  gt_boxes
+    (G,5), im_info (3,), keys int32 (H*W*A,) in (h, w, a) order; fg_inds / bg_inds / counts as
+    proposal_target returns them (MIX_INDEX) or None.  Config defaults are cfg.TRAIN's
+    (lib/mnc_config.py:75-98).  -> (labels (1,1,A*H,W), bbox_targets, bbox_inside_weights,
+    bbox_outside_weights (1,4A,H,W))."""
+    dev = gt_boxes.device
+    A = 9
+    if keys.numel() != H * W * A:
+        raise ValueError("anchor_target: keys must hold one key per anchor")
+    if (fg_inds is None) != (counts is None) or (bg_inds is None) != (counts is None):
+        raise ValueError("anchor_target: give fg_inds, bg_inds and counts together")
+    G = gt_boxes.shape[0]
+    ws = torch.empty(int(lib.mnc_anchor_target_workspace_bytes(c_int(H), c_int(W), c_int(G))),
+                     dtype=torch.uint8, device=dev)
+    labels = torch.empty((1, 1, A * H, W), dtype=torch.float32, device=dev)
+    t = [torch.empty((1, 4 * A, H, W), dtype=torch.float32, device=dev) for _ in range(3)]
+    cap = fg_inds.numel() if fg_inds is not None else 0
+    check(lib.mnc_anchor_target(
+        c_int(H), c_int(W), c_int(feat_stride), c_int(allowed_border), ptr(_f32(gt_boxes)), c_int(G),
+        ptr(_f32(im_info)), ptr(keys.contiguous().to(torch.int32)),
+        ptr(None if fg_inds is None else _f32(fg_inds)), ptr(None if bg_inds is None else _f32(bg_inds)),
+        ptr(counts), c_int(cap), c_double(negative_overlap), c_double(positive_overlap),
+        c_int(int(bool(clobber_positives))), c_double(fg_fraction), c_int(batch_size),
+        c_double(positive_weight), (ctypes.c_float * 4)(*[float(x) for x in inside_weights]),
+        ptr(ws), ptr(labels), *[ptr(x) for x in t], cur_stream()), "mnc_anchor_target", launches=5)
+    return (labels, *t)
