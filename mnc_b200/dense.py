@@ -3,11 +3,9 @@
 Activations and weights are "split" tensors: a torch bf16 tensor of shape [2, ...] holding the
 (hi, lo) planes with x ~= hi + lo.
 """
-import ctypes
-
 import torch
 
-from ._lib import lib, ptr, cur_stream, check, c_int, c_ll
+from ._lib import lib, ptr, cur_stream, check
 
 
 def split(x):
@@ -144,12 +142,10 @@ def igemm2(a, batch, H, W, cin, w, cout, taps, bias=None, relu=False, out=None, 
         ev0 = torch.cuda.Event(enable_timing=True)
         ev1 = torch.cuda.Event(enable_timing=True)
         ev0.record()
-    rc = lib.mnc_igemm_tc2(c_int(int(tri_in)), ptr(ap[0]), ptr(ap[1]), ptr(ap[2]), c_int(batch),
-                           c_int(H), c_int(W), c_int(cin), ptr(wp[0]), ptr(wp[1]), ptr(wp[2]),
-                           c_int(cout), c_int(taps), ptr(bias), c_int(int(relu)), c_int(mode),
-                           ptr(op[0]), ptr(op[1]), ptr(op[2]), c_ll(stride), c_int(out_ch_offset),
-                           c_int(split_k), c_ll(split_stride), c_int(bn), c_int(max_ctas),
-                           ctypes.c_float(acc_scale), ctypes.c_float(2.0 ** out_exp), ptr(amax),
+    rc = lib.mnc_igemm_tc2(int(tri_in), ptr(ap[0]), ptr(ap[1]), ptr(ap[2]), batch, H, W, cin,
+                           ptr(wp[0]), ptr(wp[1]), ptr(wp[2]), cout, taps, ptr(bias), int(relu),
+                           mode, ptr(op[0]), ptr(op[1]), ptr(op[2]), stride, out_ch_offset, split_k,
+                           split_stride, bn, max_ctas, acc_scale, 2.0 ** out_exp, ptr(amax),
                            cur_stream())
     check(rc, "mnc_igemm_tc2")
     if timer is not None:
@@ -199,11 +195,9 @@ def igemm(a, batch, H, W, cin, w, cout, taps, bias=None, relu=False, out=None, o
         ev1 = torch.cuda.Event(enable_timing=True)
         ev0.record()
     if impl == "tc":
-        rc = lib.mnc_igemm_tc(ptr(a[0]), ptr(a[1]), c_int(batch), c_int(H), c_int(W), c_int(cin),
-                              ptr(w[0]), ptr(w[1]), c_int(cout), c_int(taps), ptr(bias),
-                              c_int(int(relu)), c_int(mode), ptr(o0), ptr(o1), c_ll(stride),
-                              c_int(out_ch_offset), c_int(split_k), c_ll(split_stride), c_int(bn),
-                              c_int(max_ctas), cur_stream())
+        rc = lib.mnc_igemm_tc(ptr(a[0]), ptr(a[1]), batch, H, W, cin, ptr(w[0]), ptr(w[1]), cout,
+                              taps, ptr(bias), int(relu), mode, ptr(o0), ptr(o1), stride,
+                              out_ch_offset, split_k, split_stride, bn, max_ctas, cur_stream())
         check(rc, "mnc_igemm_tc")
         if timer is not None:
             ev1.record()
@@ -220,10 +214,9 @@ def igemm(a, batch, H, W, cin, w, cout, taps, bias=None, relu=False, out=None, o
                 bytes=4.0 * (batch * H * W * cin + cout * taps * cin + m_out * cout * max(split_k, 1))))
     else:
         assert split_k == 1
-        rc = lib.mnc_igemm_simt(ptr(a[0]), ptr(a[1]), c_int(batch), c_int(H), c_int(W),
-                                c_int(cin), ptr(w[0]), ptr(w[1]), c_int(cout), c_int(taps),
-                                ptr(bias), c_int(int(relu)), c_int(mode), ptr(o0), ptr(o1),
-                                c_ll(stride), c_int(out_ch_offset), cur_stream())
+        rc = lib.mnc_igemm_simt(ptr(a[0]), ptr(a[1]), batch, H, W, cin, ptr(w[0]), ptr(w[1]), cout,
+                                taps, ptr(bias), int(relu), mode, ptr(o0), ptr(o1), stride,
+                                out_ch_offset, cur_stream())
         check(rc, "mnc_igemm_simt")
 
 
@@ -234,17 +227,16 @@ def splitk_reduce(partial, splits, split_stride, rows, cols, bias=None, relu=Fal
     else:
         mode, o0, o1 = 0, out[0], out[1]
     stride = out_row_stride if out_row_stride is not None else cols
-    rc = lib.mnc_splitk_reduce(ptr(partial), c_int(splits), c_ll(split_stride), c_ll(rows),
-                               c_int(cols), ptr(bias), c_int(int(relu)), c_int(mode), ptr(o0),
-                               ptr(o1), c_ll(stride), c_int(out_ch_offset), cur_stream())
+    rc = lib.mnc_splitk_reduce(ptr(partial), splits, split_stride, rows, cols, ptr(bias), int(relu),
+                               mode, ptr(o0), ptr(o1), stride, out_ch_offset, cur_stream())
     check(rc, "mnc_splitk_reduce")
 
 
 def conv1_1(data, weight, bias, out):
     b, c, H, W = data.shape
     assert c == 3 and data.dtype == torch.float32
-    rc = lib.mnc_conv1_1(ptr(data), c_int(b), c_int(H), c_int(W), ptr(weight), ptr(bias),
-                         c_int(weight.shape[0]), ptr(out[0]), ptr(out[1]), cur_stream())
+    rc = lib.mnc_conv1_1(ptr(data), b, H, W, ptr(weight), ptr(bias), weight.shape[0], ptr(out[0]),
+                         ptr(out[1]), cur_stream())
     check(rc, "mnc_conv1_1")
 
 
@@ -267,15 +259,14 @@ def conv1_1_tc(data, w_stacked, bias, out, out_exp=0, amax=None):
         mode, op = 4, (out.h, out.l, out.c)
     else:
         mode, op = 0, (out[0], out[1], None)
-    rc = lib.mnc_conv1_1_tc2(ptr(data), c_int(b), c_int(H), c_int(W), ptr(w_stacked), ptr(bias),
-                             c_int(mode), ptr(op[0]), ptr(op[1]), ptr(op[2]),
-                             ctypes.c_float(2.0 ** out_exp), ptr(amax), cur_stream())
+    rc = lib.mnc_conv1_1_tc2(ptr(data), b, H, W, ptr(w_stacked), ptr(bias), mode, ptr(op[0]),
+                             ptr(op[1]), ptr(op[2]), 2.0 ** out_exp, ptr(amax), cur_stream())
     check(rc, "mnc_conv1_1_tc2")
 
 
 def maxpool2x2(a, batch, H, W, C, out):
-    rc = lib.mnc_maxpool2x2_split(ptr(a[0]), ptr(a[1]), c_int(batch), c_int(H), c_int(W), c_int(C),
-                                  ptr(out[0]), ptr(out[1]), cur_stream())
+    rc = lib.mnc_maxpool2x2_split(ptr(a[0]), ptr(a[1]), batch, H, W, C, ptr(out[0]), ptr(out[1]),
+                                  cur_stream())
     check(rc, "mnc_maxpool2x2_split")
 
 
@@ -283,15 +274,13 @@ def split_to_nchw(a, batch, H, W, C, out):
     if isinstance(a, Tri):     # blob read-back path (not hot): torch does the layout change
         out.copy_(a.float().view(batch, H, W, C).permute(0, 3, 1, 2))
         return
-    rc = lib.mnc_split_to_nchw(ptr(a[0]), ptr(a[1]), c_int(batch), c_int(H), c_int(W), c_int(C),
-                               ptr(out), cur_stream())
+    rc = lib.mnc_split_to_nchw(ptr(a[0]), ptr(a[1]), batch, H, W, C, ptr(out), cur_stream())
     check(rc, "mnc_split_to_nchw")
 
 
 def nchw_to_split(x, out):
     b, C, H, W = x.shape
-    rc = lib.mnc_nchw_to_split(ptr(x), c_int(b), c_int(C), c_int(H), c_int(W), ptr(out[0]),
-                               ptr(out[1]), cur_stream())
+    rc = lib.mnc_nchw_to_split(ptr(x), b, C, H, W, ptr(out[0]), ptr(out[1]), cur_stream())
     check(rc, "mnc_nchw_to_split")
 
 
@@ -299,19 +288,18 @@ def split_to_f32(a, out):
     """out (fp32, same element order) = hi + lo (split bf16) or (h + l / 2^6) * 2^-exp (Tri)."""
     n = out.numel()
     if isinstance(a, Tri):
-        rc = lib.mnc_tri_to_f32(ptr(a.h), ptr(a.l), c_ll(n), ctypes.c_float(2.0 ** -a.exp), ptr(out),
-                                cur_stream())
+        rc = lib.mnc_tri_to_f32(ptr(a.h), ptr(a.l), n, 2.0 ** -a.exp, ptr(out), cur_stream())
         check(rc, "mnc_tri_to_f32")
         return
-    rc = lib.mnc_split_to_f32(ptr(a[0]), ptr(a[1]), c_ll(n), ptr(out), cur_stream())
+    rc = lib.mnc_split_to_f32(ptr(a[0]), ptr(a[1]), n, ptr(out), cur_stream())
     check(rc, "mnc_split_to_f32")
 
 
 def f32_to_tri(x, out, exp, amax=None):
     """Device conversion fp32 -> Tri `out` (same element order) with exponent exp."""
     out.exp = int(exp)
-    rc = lib.mnc_f32_to_tri(ptr(x), c_ll(x.numel()), ctypes.c_float(2.0 ** exp), ptr(out.h), ptr(out.l),
-                            ptr(out.c), ptr(amax), cur_stream())
+    rc = lib.mnc_f32_to_tri(ptr(x), x.numel(), 2.0 ** exp, ptr(out.h), ptr(out.l), ptr(out.c),
+                            ptr(amax), cur_stream())
     check(rc, "mnc_f32_to_tri")
 
 
@@ -319,8 +307,7 @@ def splitk_reduce_tri(partial, splits, split_stride, rows, cols, out, out_exp, b
                       out_row_stride=None, out_ch_offset=0, amax=None):
     out.exp = int(out_exp)
     stride = out_row_stride if out_row_stride is not None else cols
-    rc = lib.mnc_splitk_reduce_tri(ptr(partial), c_int(splits), c_ll(split_stride), c_ll(rows),
-                                   c_int(cols), ptr(bias), c_int(int(relu)),
-                                   ctypes.c_float(2.0 ** out_exp), ptr(out.h), ptr(out.l), ptr(out.c),
-                                   c_ll(stride), c_int(out_ch_offset), ptr(amax), cur_stream())
+    rc = lib.mnc_splitk_reduce_tri(ptr(partial), splits, split_stride, rows, cols, ptr(bias),
+                                   int(relu), 2.0 ** out_exp, ptr(out.h), ptr(out.l), ptr(out.c),
+                                   stride, out_ch_offset, ptr(amax), cur_stream())
     check(rc, "mnc_splitk_reduce_tri")

@@ -20,7 +20,6 @@ def gpu_nms(dets, thresh, device_id=0):
     keep = np.zeros(boxes_num, dtype=np.int32)
     num_out = ctypes.c_int(0)
     check(lib.mnc_gpu_nms_host(keep.ctypes.data_as(ctypes.c_void_p), ctypes.byref(num_out),
-                               dets.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(boxes_num),
-                               ctypes.c_int(boxes_dim), ctypes.c_float(thresh),
-                               ctypes.c_int(device_id)), "mnc_gpu_nms_host")
+                               dets.ctypes.data_as(ctypes.c_void_p), boxes_num, boxes_dim, thresh,
+                               device_id), "mnc_gpu_nms_host")
     return [int(i) for i in keep[:num_out.value]]

@@ -30,10 +30,8 @@ def mv(all_boxes, all_masks, candidate_inds, candidate_start, candidate_weights,
     result_num = candidate_start.shape[0]
     result_mask = np.zeros((result_num, 1, all_masks.shape[2], all_masks.shape[3]), dtype=np.float32)
     result_box = np.zeros((result_num, boxes_dim), dtype=np.int32)
-    check(lib.mnc_mv_host(_p(all_boxes), _p(all_masks), ctypes.c_int(all_box_num),
-                          _p(candidate_inds), _p(candidate_start), _p(candidate_weights),
-                          ctypes.c_int(candidate_num), ctypes.c_int(int(image_height)),
-                          ctypes.c_int(int(image_width)), ctypes.c_int(boxes_dim),
-                          ctypes.c_int(mask_size), ctypes.c_int(result_num), _p(result_mask),
-                          _p(result_box), ctypes.c_int(device_id)), "mnc_mv_host")
+    check(lib.mnc_mv_host(_p(all_boxes), _p(all_masks), all_box_num, _p(candidate_inds),
+                          _p(candidate_start), _p(candidate_weights), candidate_num,
+                          int(image_height), int(image_width), boxes_dim, mask_size, result_num,
+                          _p(result_mask), _p(result_box), device_id), "mnc_mv_host")
     return result_mask, result_box

@@ -13,8 +13,8 @@ def bbox_overlaps(boxes, query_boxes):
     query_boxes = np.ascontiguousarray(query_boxes)
     N, K = boxes.shape[0], query_boxes.shape[0]
     overlaps = np.zeros((N, K), dtype=np.float64)
-    check(lib.mnc_bbox_overlaps_host(boxes.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(N),
-                                     query_boxes.ctypes.data_as(ctypes.c_void_p), ctypes.c_int(K),
+    check(lib.mnc_bbox_overlaps_host(boxes.ctypes.data_as(ctypes.c_void_p), N,
+                                     query_boxes.ctypes.data_as(ctypes.c_void_p), K,
                                      overlaps.ctypes.data_as(ctypes.c_void_p)),
           "mnc_bbox_overlaps_host")
     return overlaps

@@ -7,10 +7,7 @@ import ctypes
 
 import torch
 
-from ._lib import lib, ptr, cur_stream, check, c_int, c_ll, c_float
-
-c_double = ctypes.c_double
-lib.mnc_nms_workspace_bytes.restype = ctypes.c_longlong
+from ._lib import lib, ptr, cur_stream, check
 
 
 def _i32(*shape, device):
@@ -24,9 +21,9 @@ def rank_sort_desc(keys, n, problems, outer_stride, inner_stride=0, inner=1, key
     dev = keys.device
     order = _i32(problems, n, device=dev)
     n_valid = _i32(problems, device=dev)
-    check(lib.mnc_rank_sort_desc(ptr(keys), c_ll(outer_stride), c_ll(inner_stride), c_int(inner),
-                                 c_int(key_stride), ptr(valid), c_int(n), c_int(problems),
-                                 ptr(order), ptr(n_valid), cur_stream()), "mnc_rank_sort_desc")
+    check(lib.mnc_rank_sort_desc(ptr(keys), outer_stride, inner_stride, inner, key_stride,
+                                 ptr(valid), n, problems, ptr(order), ptr(n_valid),
+                                 cur_stream()), "mnc_rank_sort_desc")
     return order, n_valid
 
 
@@ -38,10 +35,9 @@ def topk_sort_desc(keys, n, problems, k, outer_stride, inner_stride=0, inner=1, 
     kk = min(k, n)
     order = _i32(problems, kk, device=dev)
     n_out = _i32(problems, device=dev)
-    check(lib.mnc_topk_sort_desc(ptr(keys), c_ll(outer_stride), c_ll(inner_stride), c_int(inner),
-                                 c_int(key_stride), ptr(valid), c_int(n), c_int(problems), c_int(kk),
-                                 ptr(order), c_int(kk), ptr(n_out), cur_stream()),
-          "mnc_topk_sort_desc")
+    check(lib.mnc_topk_sort_desc(ptr(keys), outer_stride, inner_stride, inner, key_stride,
+                                 ptr(valid), n, problems, kk, ptr(order), kk, ptr(n_out),
+                                 cur_stream()), "mnc_topk_sort_desc")
     return order, n_out
 
 
@@ -50,10 +46,9 @@ def gather_boxes(src, src_stride, src_outer_stride, inner, order, counts, n_out,
     dev = src.device
     dst = torch.zeros((problems, n_out, 4), dtype=torch.float32, device=dev)
     out_counts = _i32(problems, device=dev)
-    check(lib.mnc_gather_boxes(ptr(src), c_int(src_stride), c_ll(src_outer_stride), c_int(inner),
-                               ptr(order), c_int(order.shape[1]), ptr(counts), c_int(n_out),
-                               c_int(problems), ptr(dst), ptr(out_counts), cur_stream()),
-          "mnc_gather_boxes")
+    check(lib.mnc_gather_boxes(ptr(src), src_stride, src_outer_stride, inner, ptr(order),
+                               order.shape[1], ptr(counts), n_out, problems, ptr(dst),
+                               ptr(out_counts), cur_stream()), "mnc_gather_boxes")
     return dst, out_counts
 
 
@@ -65,7 +60,7 @@ def nms_sorted(boxes, counts, thresh, max_keep):
     -> (keep int32 [problems, max_keep], num int32 [problems])."""
     problems, n_max, stride = boxes.shape
     dev = boxes.device
-    nbytes = lib.mnc_nms_workspace_bytes(c_int(n_max), c_int(problems))
+    nbytes = lib.mnc_nms_workspace_bytes(n_max, problems)
     key = (dev, nbytes)
     ws = _nms_ws.get(key)
     if ws is None:
@@ -75,10 +70,10 @@ def nms_sorted(boxes, counts, thresh, max_keep):
     mk = max_keep if max_keep > 0 else n_max
     keep = _i32(problems, mk, device=dev)
     num = _i32(problems, device=dev)
-    check(lib.mnc_nms_sorted(ptr(boxes), c_int(stride), c_ll(n_max * stride), ptr(counts),
-                             c_int(n_max), c_int(problems), c_float(thresh), c_int(mk), ptr(ws),
-                             ptr(keep), c_int(mk), ptr(num), cur_stream()), "mnc_nms_sorted",
-          launches=lib.mnc_nms_sorted_launches(c_int(n_max), c_int(mk)))
+    check(lib.mnc_nms_sorted(ptr(boxes), stride, n_max * stride, ptr(counts), n_max, problems,
+                             thresh, mk, ptr(ws), ptr(keep), mk, ptr(num),
+                             cur_stream()), "mnc_nms_sorted",
+          launches=lib.mnc_nms_sorted_launches(n_max, mk))
     return keep, num
 
 
@@ -91,7 +86,7 @@ def nms_set_lazy(mode):
     per problem; 0 / False = always the suppression-matrix pair (nms_mask + nms_scan); True = the
     library default.  Returns the previous mode (int)."""
     mode = DEFAULT_NMS_MODE if mode is True else (0 if mode is False else int(mode))
-    return int(lib.mnc_nms_set_lazy(c_int(mode)))
+    return int(lib.mnc_nms_set_lazy(mode))
 
 
 # ----------------------------------------------------------------------------- proposal pieces
@@ -119,12 +114,10 @@ def rpn_decode(cls, bbox, im_info, batch, H, W, layout, apply_softmax, feat_stri
         cpad = cls.shape[-1]
         ci, cc, cp = H * W * cpad, 1, cpad
         bi, bc, bp = ci, cc, cp
-        bptr = ctypes.c_void_p(cls.data_ptr() + 18 * 4)
-    check(lib.mnc_rpn_decode(ptr(cls), c_ll(ci), c_ll(cc), c_ll(cp), bptr, c_ll(bi), c_ll(bc),
-                             c_ll(bp), ptr(im_info), c_int(batch), c_int(H), c_int(W),
-                             c_int(feat_stride), c_float(min_size), c_int(int(apply_softmax)),
-                             ptr(proposals), ptr(scores), ptr(valid), cur_stream()),
-          "mnc_rpn_decode")
+        bptr = cls.data_ptr() + 18 * 4
+    check(lib.mnc_rpn_decode(ptr(cls), ci, cc, cp, bptr, bi, bc, bp, ptr(im_info), batch, H, W,
+                             feat_stride, min_size, int(apply_softmax), ptr(proposals), ptr(scores),
+                             ptr(valid), cur_stream()), "mnc_rpn_decode")
     return proposals, scores, valid
 
 
@@ -133,10 +126,9 @@ def write_rois(sorted_boxes, keep, num_keep, max_rois, batch_index_mode):
     dev = sorted_boxes.device
     rois = torch.empty((batch, max_rois, 5), dtype=torch.float32, device=dev)
     counts = _i32(batch, device=dev)
-    check(lib.mnc_write_rois(ptr(sorted_boxes), c_int(n_sorted), ptr(keep), c_int(keep.shape[1]),
-                             ptr(num_keep), c_int(max_rois), c_int(batch),
-                             c_int(int(batch_index_mode)), ptr(rois), ptr(counts), cur_stream()),
-          "mnc_write_rois")
+    check(lib.mnc_write_rois(ptr(sorted_boxes), n_sorted, ptr(keep), keep.shape[1], ptr(num_keep),
+                             max_rois, batch, int(batch_index_mode), ptr(rois), ptr(counts),
+                             cur_stream()), "mnc_write_rois")
     return rois, counts
 
 
@@ -166,10 +158,9 @@ def stage_bridge(rois, bbox_pred, seg_cls_prob, im_info, rois_per_img):
     """rois [T,5], bbox_pred [T,>=84] (row stride = bbox_pred.stride(0)), seg_cls_prob [T,21]."""
     total = rois.shape[0]
     out = torch.empty_like(rois)
-    check(lib.mnc_stage_bridge(ptr(rois), ptr(bbox_pred), c_int(bbox_pred.stride(0)),
-                               ptr(seg_cls_prob), c_int(seg_cls_prob.stride(0)),
-                               c_int(seg_cls_prob.shape[1]), ptr(im_info), c_int(rois_per_img),
-                               c_int(total), ptr(out), cur_stream()), "mnc_stage_bridge")
+    check(lib.mnc_stage_bridge(ptr(rois), ptr(bbox_pred), bbox_pred.stride(0), ptr(seg_cls_prob),
+                               seg_cls_prob.stride(0), seg_cls_prob.shape[1], ptr(im_info),
+                               rois_per_img, total, ptr(out), cur_stream()), "mnc_stage_bridge")
     return out
 
 
@@ -178,16 +169,16 @@ def softmax_rows(x, cols=None, out=None):
     cols = cols or x.shape[1]
     if out is None:
         out = torch.empty((rows, cols), dtype=torch.float32, device=x.device)
-    check(lib.mnc_softmax_rows(ptr(x), c_int(x.stride(0)), c_int(rows), c_int(cols), ptr(out),
-                               c_int(out.stride(0)), cur_stream()), "mnc_softmax_rows")
+    check(lib.mnc_softmax_rows(ptr(x), x.stride(0), rows, cols, ptr(out), out.stride(0),
+                               cur_stream()), "mnc_softmax_rows")
     return out
 
 
 def unscale_clip(rois, rois_per_img, im_scale, im_hw):
     total = rois.shape[0]
     boxes = torch.empty((total, 4), dtype=torch.float32, device=rois.device)
-    check(lib.mnc_unscale_clip(ptr(rois), c_int(total), c_int(rois_per_img), ptr(im_scale),
-                               ptr(im_hw), ptr(boxes), cur_stream()), "mnc_unscale_clip")
+    check(lib.mnc_unscale_clip(ptr(rois), total, rois_per_img, ptr(im_scale), ptr(im_hw),
+                               ptr(boxes), cur_stream()), "mnc_unscale_clip")
     return boxes
 
 
@@ -215,9 +206,8 @@ def detect_tail(o, B, n, im_scale, im_hw, rec, valid):
     check(lib.mnc_detect_tail(ptr(o["rois"]), ptr(o["rois_ext"]), ptr(o["mask_proposal"]),
                               ptr(o["mask_proposal_ext"]), ptr(o["seg_cls_prob"]),
                               ptr(o["seg_cls_prob_ext"]), ptr(o["roi_counts"]), ptr(im_scale),
-                              ptr(im_hw), c_int(B), c_int(n), c_int(msz), c_int(ncls), ptr(counts),
-                              ptr(boxes), ptr(scores), ptr(masks), ptr(valid), cur_stream()),
-          "mnc_detect_tail")
+                              ptr(im_hw), B, n, msz, ncls, ptr(counts), ptr(boxes), ptr(scores),
+                              ptr(masks), ptr(valid), cur_stream()), "mnc_detect_tail")
     return counts, boxes, scores, masks
 
 
@@ -225,9 +215,9 @@ def decode_class_boxes(rois, bbox_pred, rois_per_img, im_scale, im_hw, ncls=21):
     """-> (R, ncls*4) fp32: per-class decoded boxes in original-image coordinates, clipped."""
     R = rois.shape[0]
     out = torch.empty((R, ncls * 4), dtype=torch.float32, device=rois.device)
-    check(lib.mnc_decode_class_boxes(ptr(rois), c_int(R), c_int(rois_per_img), ptr(bbox_pred),
-                                     c_int(bbox_pred.stride(0)), c_int(ncls), ptr(im_scale),
-                                     ptr(im_hw), ptr(out), cur_stream()), "mnc_decode_class_boxes")
+    check(lib.mnc_decode_class_boxes(ptr(rois), R, rois_per_img, ptr(bbox_pred),
+                                     bbox_pred.stride(0), ncls, ptr(im_scale), ptr(im_hw), ptr(out),
+                                     cur_stream()), "mnc_decode_class_boxes")
     return out
 
 
@@ -237,17 +227,16 @@ def roi_warp_nchw(feat, rois, pooled_h, pooled_w, spatial_scale=0.0625, out=None
     R = rois.shape[0]
     if out is None:
         out = torch.empty((R, C, pooled_h, pooled_w), dtype=torch.float32, device=feat.device)
-    check(lib.mnc_roi_warp_nchw(ptr(feat), c_int(C), c_int(H), c_int(W), ptr(rois), c_int(R),
-                                c_int(pooled_h), c_int(pooled_w), c_float(spatial_scale), ptr(out),
-                                cur_stream()), "mnc_roi_warp_nchw")
+    check(lib.mnc_roi_warp_nchw(ptr(feat), C, H, W, ptr(rois), R, pooled_h, pooled_w, spatial_scale,
+                                ptr(out), cur_stream()), "mnc_roi_warp_nchw")
     return out
 
 
 def mask_resize_nchw(x, out_h, out_w):
     N, C, ih, iw = x.shape
     out = torch.empty((N, C, out_h, out_w), dtype=torch.float32, device=x.device)
-    check(lib.mnc_mask_resize_nchw(ptr(x), c_int(N), c_int(C), c_int(ih), c_int(iw), c_int(out_h),
-                                   c_int(out_w), ptr(out), cur_stream()), "mnc_mask_resize_nchw")
+    check(lib.mnc_mask_resize_nchw(ptr(x), N, C, ih, iw, out_h, out_w, ptr(out),
+                                   cur_stream()), "mnc_mask_resize_nchw")
     return out
 
 
@@ -258,8 +247,8 @@ def mask_pool_nchw(feat, mask, out=None):
                          "(mask_pooling_layer.cpp:20-29)")
     if out is None:
         out = torch.empty_like(feat)
-    check(lib.mnc_mask_pool_nchw(ptr(feat), ptr(mask), c_int(N), c_int(C), c_int(H), c_int(W),
-                                 ptr(out), cur_stream()), "mnc_mask_pool_nchw")
+    check(lib.mnc_mask_pool_nchw(ptr(feat), ptr(mask), N, C, H, W, ptr(out),
+                                 cur_stream()), "mnc_mask_pool_nchw")
     return out
 
 
@@ -267,8 +256,7 @@ def roi_warp_split(feat, C, H, W, rois, sub, out14, out7, spatial_scale=0.0625):
     """feat fp32 NHWC [B,H,W,C]; rois [R,5]; out14 split [2,R,14,14,C]; out7 split [2,R,7,7,C]."""
     R = rois.shape[0]
     assert feat.dtype == torch.float32
-    check(lib.mnc_roi_warp_split(ptr(feat), c_int(C), c_int(H), c_int(W),
-                                 ptr(rois), c_int(R), c_int(sub), c_float(spatial_scale),
+    check(lib.mnc_roi_warp_split(ptr(feat), C, H, W, ptr(rois), R, sub, spatial_scale,
                                  ptr(out14[0]), ptr(out14[1]), ptr(out7[0]), ptr(out7[1]),
                                  cur_stream()), "mnc_roi_warp_split")
 
@@ -278,32 +266,30 @@ def roi_warp_tri(feat, C, H, W, rois, sub, out14, out7, exp, spatial_scale=0.062
     R = rois.shape[0]
     assert feat.dtype == torch.float32
     out14.exp = out7.exp = int(exp)
-    check(lib.mnc_roi_warp_tri(ptr(feat), c_int(C), c_int(H), c_int(W), ptr(rois), c_int(R), c_int(sub),
-                               c_float(spatial_scale), c_float(2.0 ** exp), ptr(out14.h), ptr(out14.l),
-                               ptr(out14.c), ptr(out7.h), ptr(out7.l), ptr(out7.c), cur_stream()),
-          "mnc_roi_warp_tri")
+    check(lib.mnc_roi_warp_tri(ptr(feat), C, H, W, ptr(rois), R, sub, spatial_scale, 2.0 ** exp,
+                               ptr(out14.h), ptr(out14.l), ptr(out14.c), ptr(out7.h), ptr(out7.l),
+                               ptr(out7.c), cur_stream()), "mnc_roi_warp_tri")
 
 
 def mask_pool_tri(feat14, mask14, R, C, out7):
     """MaskPooling + 2x2 max pool on tri-plane features; the output takes the input's exponent."""
     out7.exp = feat14.exp
-    check(lib.mnc_mask_pool_tri(ptr(feat14.h), ptr(feat14.l), ptr(mask14), c_int(R), c_int(C),
-                                ptr(out7.h), ptr(out7.l), ptr(out7.c), cur_stream()), "mnc_mask_pool_tri")
+    check(lib.mnc_mask_pool_tri(ptr(feat14.h), ptr(feat14.l), ptr(mask14), R, C, ptr(out7.h),
+                                ptr(out7.l), ptr(out7.c), cur_stream()), "mnc_mask_pool_tri")
 
 
 def sigmoid_mask_resize(logits, R, mask_size=21, out_size=14):
     dev = logits.device
     mp = torch.empty((R, 1, mask_size, mask_size), dtype=torch.float32, device=dev)
     mr = torch.empty((R, 1, out_size, out_size), dtype=torch.float32, device=dev)
-    check(lib.mnc_sigmoid_mask_resize(ptr(logits), c_int(logits.stride(0)), c_int(R),
-                                      c_int(mask_size), c_int(out_size), ptr(mp), ptr(mr),
-                                      cur_stream()), "mnc_sigmoid_mask_resize")
+    check(lib.mnc_sigmoid_mask_resize(ptr(logits), logits.stride(0), R, mask_size, out_size,
+                                      ptr(mp), ptr(mr), cur_stream()), "mnc_sigmoid_mask_resize")
     return mp, mr
 
 
 def mask_pool_split(feat14, mask14, R, C, out7):
-    check(lib.mnc_mask_pool_split(ptr(feat14[0]), ptr(feat14[1]), ptr(mask14), c_int(R), c_int(C),
-                                  ptr(out7[0]), ptr(out7[1]), cur_stream()), "mnc_mask_pool_split")
+    check(lib.mnc_mask_pool_split(ptr(feat14[0]), ptr(feat14[1]), ptr(mask14), R, C, ptr(out7[0]),
+                                  ptr(out7[1]), cur_stream()), "mnc_mask_pool_split")
 
 
 def roi_pool_nchw(feat, rois, pooled_h, pooled_w, spatial_scale=0.0625, out=None, argmax=None):
@@ -312,24 +298,23 @@ def roi_pool_nchw(feat, rois, pooled_h, pooled_w, spatial_scale=0.0625, out=None
     R = rois.shape[0]
     if out is None:
         out = torch.empty((R, C, pooled_h, pooled_w), dtype=torch.float32, device=feat.device)
-    check(lib.mnc_roi_pool_nchw(ptr(feat), c_int(C), c_int(H), c_int(W), ptr(rois), c_int(R),
-                                c_int(pooled_h), c_int(pooled_w), c_float(spatial_scale), ptr(out),
-                                ptr(argmax), cur_stream()), "mnc_roi_pool_nchw")
+    check(lib.mnc_roi_pool_nchw(ptr(feat), C, H, W, ptr(rois), R, pooled_h, pooled_w, spatial_scale,
+                                ptr(out), ptr(argmax), cur_stream()), "mnc_roi_pool_nchw")
     return out
 
 
 def roi_pool_split(feat, C, H, W, rois, pooled, out, spatial_scale=0.0625):
     """feat fp32 NHWC [B,H,W,C]; rois [R,5]; out split [2,R,P,P,C] (ROIPooling)."""
-    check(lib.mnc_roi_pool_split(ptr(feat), c_int(C), c_int(H), c_int(W), ptr(rois),
-                                 c_int(rois.shape[0]), c_int(pooled), c_float(spatial_scale),
-                                 ptr(out[0]), ptr(out[1]), cur_stream()), "mnc_roi_pool_split")
+    check(lib.mnc_roi_pool_split(ptr(feat), C, H, W, ptr(rois), rois.shape[0], pooled,
+                                 spatial_scale, ptr(out[0]), ptr(out[1]),
+                                 cur_stream()), "mnc_roi_pool_split")
 
 
 def roi_sample_split(feat, C, H, W, rois, pooled, out, spatial_scale=0.0625):
     """feat fp32 NHWC [B,H,W,C]; rois [R,5]; out split [2,R,P,P,C] (ROIWarping, no pool after)."""
-    check(lib.mnc_roi_sample_split(ptr(feat), c_int(C), c_int(H), c_int(W), ptr(rois),
-                                   c_int(rois.shape[0]), c_int(pooled), c_float(spatial_scale),
-                                   ptr(out[0]), ptr(out[1]), cur_stream()), "mnc_roi_sample_split")
+    check(lib.mnc_roi_sample_split(ptr(feat), C, H, W, ptr(rois), rois.shape[0], pooled,
+                                   spatial_scale, ptr(out[0]), ptr(out[1]),
+                                   cur_stream()), "mnc_roi_sample_split")
 
 
 # ----------------------------------------------------------------------------- layer backward passes
@@ -342,9 +327,8 @@ def roi_warp_backward_nchw(feat, rois, top_diff, pooled_h, pooled_w, spatial_sca
     new = torch.zeros if R == 0 else torch.empty       # R = 0: the library writes nothing
     fd = new(feat.shape, dtype=torch.float32, device=feat.device) if want_feat else None
     rd = new((R, 5), dtype=torch.float32, device=feat.device) if want_rois else None
-    check(lib.mnc_roi_warp_backward_nchw(ptr(feat), c_int(B), c_int(C), c_int(H), c_int(W), ptr(rois),
-                                         c_int(R), c_int(pooled_h), c_int(pooled_w),
-                                         c_float(spatial_scale), ptr(top_diff), ptr(fd), ptr(rd),
+    check(lib.mnc_roi_warp_backward_nchw(ptr(feat), B, C, H, W, ptr(rois), R, pooled_h, pooled_w,
+                                         spatial_scale, ptr(top_diff), ptr(fd), ptr(rd),
                                          cur_stream()), "mnc_roi_warp_backward_nchw",
           launches=int(want_feat) + 2 * int(want_rois))
     return fd, rd
@@ -354,9 +338,8 @@ def mask_resize_backward_nchw(top_diff, in_h, in_w):
     """MaskResizeLayer backward (mask_resize_layer.cu:135-183): top_diff (N,C,oh,ow) -> (N,C,in_h,in_w)."""
     N, C, oh, ow = top_diff.shape
     out = torch.empty((N, C, in_h, in_w), dtype=torch.float32, device=top_diff.device)
-    check(lib.mnc_mask_resize_backward_nchw(ptr(top_diff), c_int(N), c_int(C), c_int(in_h), c_int(in_w),
-                                            c_int(oh), c_int(ow), ptr(out), cur_stream()),
-          "mnc_mask_resize_backward_nchw")
+    check(lib.mnc_mask_resize_backward_nchw(ptr(top_diff), N, C, in_h, in_w, oh, ow, ptr(out),
+                                            cur_stream()), "mnc_mask_resize_backward_nchw")
     return out
 
 
@@ -368,8 +351,8 @@ def mask_pool_backward_nchw(feat, mask, top_diff, want_feat=True, want_mask=True
                          "(mask_pooling_layer.cpp:20-29)")
     fd = torch.empty_like(feat) if want_feat else None
     md = torch.empty_like(mask) if want_mask else None
-    check(lib.mnc_mask_pool_backward_nchw(ptr(feat), ptr(mask), ptr(top_diff), c_int(N), c_int(C),
-                                          c_int(H), c_int(W), ptr(fd), ptr(md), cur_stream()),
+    check(lib.mnc_mask_pool_backward_nchw(ptr(feat), ptr(mask), ptr(top_diff), N, C, H, W, ptr(fd),
+                                          ptr(md), cur_stream()),
           "mnc_mask_pool_backward_nchw", launches=int(want_feat) + int(want_mask))
     return fd, md
 
@@ -382,9 +365,8 @@ def roi_pool_backward_nchw(top_diff, argmax, feat_shape, rois, pooled_h, pooled_
     R = rois.shape[0]
     new = torch.zeros if R == 0 else torch.empty
     out = new((B, C, H, W), dtype=torch.float32, device=top_diff.device)
-    check(lib.mnc_roi_pool_backward_nchw(ptr(top_diff), ptr(argmax), c_int(B), c_int(C), c_int(H),
-                                         c_int(W), ptr(rois), c_int(R), c_int(pooled_h),
-                                         c_int(pooled_w), c_float(spatial_scale), ptr(out),
+    check(lib.mnc_roi_pool_backward_nchw(ptr(top_diff), ptr(argmax), B, C, H, W, ptr(rois), R,
+                                         pooled_h, pooled_w, spatial_scale, ptr(out),
                                          cur_stream()), "mnc_roi_pool_backward_nchw")
     return out
 
@@ -420,28 +402,25 @@ def mask_voting(boxes, masks, scores, im_hw, max_per_image=100, nms_thresh=0.3, 
     n_res = _i32(B, device=dev)
     class_bar = _i32(B, ncls - 1, device=dev)
     overflow = torch.zeros(1, dtype=torch.int32, device=dev)
-    check(lib.mnc_vote_select(ptr(scores), c_int(nb), c_int(ncls), ptr(order), ptr(keep),
-                              c_int(keep.shape[1]), ptr(num), c_int(max_per_image),
-                              c_int(max_results), c_int(B), ptr(res_idx), ptr(res_cls),
+    check(lib.mnc_vote_select(ptr(scores), nb, ncls, ptr(order), ptr(keep), keep.shape[1], ptr(num),
+                              max_per_image, max_results, B, ptr(res_idx), ptr(res_cls),
                               ptr(res_score), ptr(n_res), ptr(class_bar), ptr(overflow),
                               cur_stream()), "mnc_vote_select")
     cand_inds = _i32(B, max_results, nb, device=dev)
     cand_w = torch.empty((B, max_results, nb), dtype=torch.float32, device=dev)   # lists only; gaps unread
     cand_begin = _i32(B, max_results, device=dev)
     cand_end = _i32(B, max_results, device=dev)
-    check(lib.mnc_vote_candidates(ptr(boxes), ptr(scores), ptr(box_valid), c_int(nb), c_int(ncls),
-                                  ptr(res_idx),
-                                  ptr(res_cls), ptr(n_res), c_int(max_results), c_int(B),
-                                  c_double(iou_thresh), ptr(cand_inds), ptr(cand_w),
-                                  ptr(cand_begin), ptr(cand_end), cur_stream()),
-          "mnc_vote_candidates")
+    check(lib.mnc_vote_candidates(ptr(boxes), ptr(scores), ptr(box_valid), nb, ncls, ptr(res_idx),
+                                  ptr(res_cls), ptr(n_res), max_results, B, iou_thresh,
+                                  ptr(cand_inds), ptr(cand_w), ptr(cand_begin), ptr(cand_end),
+                                  cur_stream()), "mnc_vote_candidates")
     bbox_ws = _i32(B * max_results * 4 + B, device=dev)   # tight boxes + per-image range flag
     out_mask = torch.zeros((B, max_results, 1, M, M), dtype=torch.float32, device=dev)
     out_box = torch.zeros((B, max_results, 4), dtype=torch.int32, device=dev)
-    check(lib.mnc_mv_device(ptr(boxes), ptr(masks), c_int(nb), c_int(4), c_int(M), ptr(cand_inds),
-                            ptr(cand_w), c_ll(max_results * nb), ptr(cand_begin), ptr(cand_end),
-                            ptr(n_res), c_int(max_results), c_int(B), ptr(im_hw), ptr(bbox_ws),
-                            ptr(out_mask), ptr(out_box), cur_stream()), "mnc_mv_device",
+    check(lib.mnc_mv_device(ptr(boxes), ptr(masks), nb, 4, M, ptr(cand_inds), ptr(cand_w),
+                            max_results * nb, ptr(cand_begin), ptr(cand_end), ptr(n_res),
+                            max_results, B, ptr(im_hw), ptr(bbox_ws), ptr(out_mask), ptr(out_box),
+                            cur_stream()), "mnc_mv_device",
           launches=lib.mnc_mv_device_launches())
     return dict(n_res=n_res, class_bar=class_bar, res_score=res_score, res_class=res_cls,
                 res_box_idx=res_idx, result_mask=out_mask, result_box=out_box,
@@ -452,7 +431,7 @@ def mask_voting(boxes, masks, scores, im_hw, max_per_image=100, nms_thresh=0.3, 
 def mv_set_two_pass(on):
     """A/B and cross-check switch of mnc_mv_device: False = one full sweep of each result's region
     instead of the coarse pass + exact border pass.  Returns the previous setting."""
-    return bool(lib.mnc_mv_set_two_pass(c_int(1 if on else 0)))
+    return bool(lib.mnc_mv_set_two_pass(1 if on else 0))
 
 
 def mask_voting_checked(boxes, masks, scores, im_hw, max_per_image=100, box_valid=None, **kw):
@@ -494,8 +473,7 @@ def prep_images(images_u8, scale, out=None, pixel_means=PIXEL_MEANS):
     if out is None:
         out = torch.empty((B, 3, out_h, out_w), dtype=torch.float32, device=images_u8.device)
     means = (ctypes.c_double * 3)(*pixel_means)
-    check(lib.mnc_prep_images(ptr(images_u8), c_int(B), c_int(H), c_int(W), means,
-                              ctypes.c_double(scale), c_int(out_h), c_int(out_w), ptr(out),
+    check(lib.mnc_prep_images(ptr(images_u8), B, H, W, means, scale, out_h, out_w, ptr(out),
                               cur_stream()), "mnc_prep_images")
     return out
 
@@ -515,9 +493,8 @@ def paste_instances(boxes, masks, cls, counts, H, W, thresh=0.4, want_bgr=False)
     inst = torch.empty((B, H, W), dtype=torch.int32, device=dev)
     clsi = torch.empty((B, H, W), dtype=torch.int32, device=dev)
     bgr = torch.empty((B, H, W, 3), dtype=torch.uint8, device=dev) if want_bgr else None
-    check(lib.mnc_paste_instances(ptr(boxes), c_int(box_dim), ptr(masks), ptr(cls), ptr(counts),
-                                  c_int(B), c_int(n), c_int(M), c_int(H), c_int(W), c_float(thresh),
-                                  ptr(inst), ptr(clsi), ptr(bgr), cur_stream()),
+    check(lib.mnc_paste_instances(ptr(boxes), box_dim, ptr(masks), ptr(cls), ptr(counts), B, n, M,
+                                  H, W, thresh, ptr(inst), ptr(clsi), ptr(bgr), cur_stream()),
           "mnc_paste_instances")
     return (inst, clsi, bgr) if want_bgr else (inst, clsi)
 
@@ -551,9 +528,9 @@ def binarize_masks(rboxes, masks, thresh=0.4):
     np.cumsum(areas, out=offsets[1:])
     out = torch.empty((max(int(offsets[-1]), 1),), dtype=torch.uint8, device=rboxes.device)
     d_off = torch.from_numpy(offsets[:-1].copy()).to(rboxes.device)
-    check(lib.mnc_binarize_masks(ptr(rb), ptr(masks.contiguous().float()), c_int(n), c_int(M),
-                                 c_float(thresh), ptr(d_off), c_int(int(areas.max()) if n else 0),
-                                 ptr(out), cur_stream()), "mnc_binarize_masks")
+    check(lib.mnc_binarize_masks(ptr(rb), ptr(masks.contiguous().float()), n, M, thresh, ptr(d_off),
+                                 int(areas.max()) if n else 0, ptr(out),
+                                 cur_stream()), "mnc_binarize_masks")
     return out, offsets
 
 
@@ -586,11 +563,11 @@ def stage_bridge_train(rois, bbox_pred, seg_cls_prob, gt_boxes, gt_masks, im_inf
     dbl4 = lambda v: None if v is None else (ctypes.c_double * 4)(*[float(x) for x in v])
     gm = _f32(gt_masks)
     check(lib.mnc_stage_bridge_train(
-        ptr(_f32(rois)), c_int(n), ptr(_f32(bbox_pred)), ptr(_f32(seg_cls_prob)), c_int(C),
-        ptr(_f32(gt_boxes)), c_int(G), ptr(gm), c_int(gm.shape[1]), c_int(gm.shape[2]),
-        ptr(_f32(im_info)), ptr(mask_info.contiguous().to(torch.int32)), dbl4(means), dbl4(stds),
-        (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), ctypes.c_double(bbox_thresh),
-        c_int(M), c_float(binarize_thresh), *[ptr(out[k]) for k in (
+        ptr(_f32(rois)), n, ptr(_f32(bbox_pred)), ptr(_f32(seg_cls_prob)), C, ptr(_f32(gt_boxes)),
+        G, ptr(gm), gm.shape[1], gm.shape[2], ptr(_f32(im_info)),
+        ptr(mask_info.contiguous().to(torch.int32)), dbl4(means), dbl4(stds),
+        (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), bbox_thresh, M, binarize_thresh,
+        *[ptr(out[k]) for k in (
             "rois", "labels", "mask_targets", "mask_weight", "gt_mask_info", "bbox_targets",
             "bbox_inside_weights", "bbox_outside_weights", "state")], cur_stream()),
         "mnc_stage_bridge_train", launches=2)
@@ -609,8 +586,8 @@ def stage_bridge_train_backward(top_diff, state, rois, bbox_pred, G, clip_thresh
     rd = new((n, 5), dtype=torch.float32, device=dev) if want_rois else None
     bd = new((n, C4), dtype=torch.float32, device=dev) if want_bbox else None
     check(lib.mnc_stage_bridge_train_backward(
-        ptr(_f32(top_diff)), ptr(state), ptr(_f32(rois)), ptr(_f32(bbox_pred)), c_int(n), c_int(G),
-        c_int(C4 // 4), c_float(clip_thresh), ptr(rd), ptr(bd), cur_stream()),
+        ptr(_f32(top_diff)), ptr(state), ptr(_f32(rois)), ptr(_f32(bbox_pred)), n, G, C4 // 4,
+        clip_thresh, ptr(rd), ptr(bd), cur_stream()),
         "mnc_stage_bridge_train_backward", launches=int(n > 0 and (want_rois or want_bbox)))
     return rd, bd
 
@@ -623,10 +600,10 @@ def mask_layer_train(mask_pred, gt_masks, gt_masks_info, binarize_thresh=0.4, fg
     M = int(round((mask_pred.numel() // max(N, 1)) ** 0.5)) if N else 21
     gm = _f32(gt_masks)
     labels = torch.empty((N,), dtype=torch.float32, device=mask_pred.device)
-    check(lib.mnc_mask_layer_train(ptr(_f32(mask_pred)), c_int(N), c_int(M), ptr(gm), c_int(gm.shape[0]),
-                                   c_int(gm.shape[1]), c_int(gm.shape[2]), ptr(_f32(gt_masks_info)),
-                                   c_float(binarize_thresh), ctypes.c_double(fg_seg_thresh),
-                                   ptr(labels), cur_stream()), "mnc_mask_layer_train")
+    check(lib.mnc_mask_layer_train(ptr(_f32(mask_pred)), N, M, ptr(gm), gm.shape[0], gm.shape[1],
+                                   gm.shape[2], ptr(_f32(gt_masks_info)), binarize_thresh,
+                                   fg_seg_thresh, ptr(labels),
+                                   cur_stream()), "mnc_mask_layer_train")
     return labels
 
 
@@ -636,16 +613,12 @@ def mask_layer_train_backward(top_diff, labels):
     N = top_diff.shape[0]
     M = top_diff.shape[-1]
     out = torch.empty((N, M * M), dtype=torch.float32, device=top_diff.device)
-    check(lib.mnc_mask_layer_train_backward(ptr(_f32(top_diff)), ptr(_f32(labels)), c_int(N), c_int(M),
-                                            ptr(out), cur_stream()), "mnc_mask_layer_train_backward")
+    check(lib.mnc_mask_layer_train_backward(ptr(_f32(top_diff)), ptr(_f32(labels)), N, M, ptr(out),
+                                            cur_stream()), "mnc_mask_layer_train_backward")
     return out
 
 
 # ------------------------------------------------------------------ training-phase RPN-stage layers
-lib.mnc_proposal_target_state_ints.restype = ctypes.c_longlong
-lib.mnc_anchor_target_workspace_bytes.restype = ctypes.c_longlong
-
-
 def sample_keys(*shape, device):
     """Random uint32 sampling keys (as int32) from torch's generator on `device`: the chosen subset
     of a category is its candidates with the smallest (key, index) pairs (include/mnc_b200.h)."""
@@ -666,9 +639,9 @@ def proposal_train(cls, bbox, im_info, H, W, pre_nms_top_n=12000, post_nms_top_n
     R = rois.shape[1]
     index = torch.empty((R,), dtype=torch.float32, device=cls.device)
     state = _i32(R, 2, device=cls.device)
-    check(lib.mnc_proposal_train_state(ptr(mid["order"]), ptr(mid["keep"]), ptr(mid["num"]), c_int(R),
-                                       ptr(bbox), c_int(H), c_int(W), c_int(feat_stride), ptr(im_info),
-                                       ptr(index), ptr(state), cur_stream()),
+    check(lib.mnc_proposal_train_state(ptr(mid["order"]), ptr(mid["keep"]), ptr(mid["num"]), R,
+                                       ptr(bbox), H, W, feat_stride, ptr(im_info), ptr(index),
+                                       ptr(state), cur_stream()),
           "mnc_proposal_train_state", launches=int(R > 0))
     return rois[0], index, counts, state
 
@@ -680,15 +653,14 @@ def proposal_backward(top_diff, state, bbox, clip_thresh=0.0):
     H, W = bbox.shape[-2:]
     out = torch.empty_like(bbox)
     R = state.shape[0]
-    check(lib.mnc_proposal_backward(ptr(_f32(top_diff)), c_int(R), ptr(state), ptr(bbox), c_int(H),
-                                    c_int(W), c_float(clip_thresh), ptr(out), cur_stream()),
+    check(lib.mnc_proposal_backward(ptr(_f32(top_diff)), R, ptr(state), ptr(bbox), H, W,
+                                    clip_thresh, ptr(out), cur_stream()),
           "mnc_proposal_backward", launches=1 + int(R > 0))
     return out
 
 
 def proposal_target_capacity(batch_size, fg_fraction, bg_fraction):
-    return int(lib.mnc_proposal_target_capacity(c_int(batch_size), c_int(len(fg_fraction)),
-                                                c_int(len(bg_fraction))))
+    return int(lib.mnc_proposal_target_capacity(batch_size, len(fg_fraction), len(bg_fraction)))
 
 
 def proposal_target(rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_info, keys,
@@ -718,21 +690,19 @@ def proposal_target(rpn_rois, rpn_rois_index, gt_boxes, gt_masks, mask_info, im_
            "mask_targets": e(Kmax, 1, M, M), "mask_weight": e(Kmax, 1, M, M),
            "gt_masks_info": e(Kmax, 12), "fg_inds": e(Kmax), "bg_inds": e(Kmax),
            "counts": _i32(4, device=dev),
-           "state": _i32(int(lib.mnc_proposal_target_state_ints(c_int(n), c_int(G), c_int(Kmax))),
-                         device=dev)}
-    dbl = lambda v: None if v is None else (c_double * len(v))(*[float(x) for x in v])
+           "state": _i32(int(lib.mnc_proposal_target_state_ints(n, G, Kmax)), device=dev)}
+    dbl = lambda v: None if v is None else (ctypes.c_double * len(v))(*[float(x) for x in v])
     gm = _f32(gt_masks)
     idx = _f32(rpn_rois_index).reshape(-1) if n else None
     check(lib.mnc_proposal_target(
-        ptr(_f32(rpn_rois)), c_int(n), ptr(idx),
+        ptr(_f32(rpn_rois)), n, ptr(idx),
         ptr(None if n_valid is None else n_valid.contiguous().to(torch.int32)), ptr(_f32(gt_boxes)),
-        c_int(G), ptr(gm),
-        c_int(gm.shape[1]), c_int(gm.shape[2]), ptr(mask_info.contiguous().to(torch.int32)),
-        ptr(_f32(im_info)), ptr(keys.contiguous().to(torch.int32)), c_int(batch_size),
-        c_int(len(fg_fraction)), dbl(fg_fraction), dbl(fg_thresh_lo), dbl(fg_thresh_hi),
-        c_int(len(bg_fraction)), dbl(bg_fraction), dbl(bg_thresh_lo), dbl(bg_thresh_hi),
-        dbl(means), dbl(stds), (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), c_int(M),
-        c_float(binarize_thresh), c_int(C), c_int(Kmax), *[ptr(out[k]) for k in (
+        G, ptr(gm), gm.shape[1], gm.shape[2], ptr(mask_info.contiguous().to(torch.int32)),
+        ptr(_f32(im_info)), ptr(keys.contiguous().to(torch.int32)), batch_size,
+        len(fg_fraction), dbl(fg_fraction), dbl(fg_thresh_lo), dbl(fg_thresh_hi),
+        len(bg_fraction), dbl(bg_fraction), dbl(bg_thresh_lo), dbl(bg_thresh_hi),
+        dbl(means), dbl(stds), (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), M,
+        binarize_thresh, C, Kmax, *[ptr(out[k]) for k in (
             "rois", "labels", "bbox_targets", "bbox_inside_weights", "bbox_outside_weights",
             "mask_targets", "mask_weight", "gt_masks_info", "fg_inds", "bg_inds", "counts",
             "state")], cur_stream()), "mnc_proposal_target", launches=2)
@@ -744,8 +714,8 @@ def proposal_target_backward(top_diff, state, n, G, bp_all=True):
     rois top -> rpn_rois diff (n,5); rows >= K of top_diff are never read."""
     dev = state.device
     out = (torch.zeros if n == 0 else torch.empty)((n, 5), dtype=torch.float32, device=dev)
-    check(lib.mnc_proposal_target_backward(ptr(_f32(top_diff)), ptr(state), c_int(n), c_int(G),
-                                           c_int(int(bool(bp_all))), ptr(out), cur_stream()),
+    check(lib.mnc_proposal_target_backward(ptr(_f32(top_diff)), ptr(state), n, G, int(bool(bp_all)),
+                                           ptr(out), cur_stream()),
           "mnc_proposal_target_backward", launches=int(n > 0))
     return out
 
@@ -766,17 +736,16 @@ def anchor_target(H, W, gt_boxes, im_info, keys, fg_inds=None, bg_inds=None, cou
     if (fg_inds is None) != (counts is None) or (bg_inds is None) != (counts is None):
         raise ValueError("anchor_target: give fg_inds, bg_inds and counts together")
     G = gt_boxes.shape[0]
-    ws = torch.empty(int(lib.mnc_anchor_target_workspace_bytes(c_int(H), c_int(W), c_int(G))),
-                     dtype=torch.uint8, device=dev)
+    ws = torch.empty(int(lib.mnc_anchor_target_workspace_bytes(H, W, G)), dtype=torch.uint8,
+                     device=dev)
     labels = torch.empty((1, 1, A * H, W), dtype=torch.float32, device=dev)
     t = [torch.empty((1, 4 * A, H, W), dtype=torch.float32, device=dev) for _ in range(3)]
     cap = fg_inds.numel() if fg_inds is not None else 0
     check(lib.mnc_anchor_target(
-        c_int(H), c_int(W), c_int(feat_stride), c_int(allowed_border), ptr(_f32(gt_boxes)), c_int(G),
-        ptr(_f32(im_info)), ptr(keys.contiguous().to(torch.int32)),
-        ptr(None if fg_inds is None else _f32(fg_inds)), ptr(None if bg_inds is None else _f32(bg_inds)),
-        ptr(counts), c_int(cap), c_double(negative_overlap), c_double(positive_overlap),
-        c_int(int(bool(clobber_positives))), c_double(fg_fraction), c_int(batch_size),
-        c_double(positive_weight), (ctypes.c_float * 4)(*[float(x) for x in inside_weights]),
-        ptr(ws), ptr(labels), *[ptr(x) for x in t], cur_stream()), "mnc_anchor_target", launches=5)
+        H, W, feat_stride, allowed_border, ptr(_f32(gt_boxes)), G, ptr(_f32(im_info)),
+        ptr(keys.contiguous().to(torch.int32)), ptr(None if fg_inds is None else _f32(fg_inds)),
+        ptr(None if bg_inds is None else _f32(bg_inds)), ptr(counts), cap, negative_overlap,
+        positive_overlap, int(bool(clobber_positives)), fg_fraction, batch_size, positive_weight,
+        (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), ptr(ws), ptr(labels),
+        ptr(t[0]), ptr(t[1]), ptr(t[2]), cur_stream()), "mnc_anchor_target", launches=5)
     return (labels, *t)

@@ -30,8 +30,8 @@ def test_nms_host_matches_oracle(n, thresh):
     keep = np.zeros(n, dtype=np.int32)
     num = ctypes.c_int(0)
     check(lib.mnc_nms_host(keep.ctypes.data_as(ctypes.c_void_p), ctypes.byref(num),
-                           sorted_dets.ctypes.data_as(ctypes.c_void_p), n, 5,
-                           ctypes.c_float(thresh), 0), "mnc_nms_host")
+                           sorted_dets.ctypes.data_as(ctypes.c_void_p), n, 5, thresh, 0),
+          "mnc_nms_host")
     got = keep[:num.value]
     assert num.value == len(want)
     assert np.array_equal(got, want)

@@ -47,7 +47,7 @@ def test_roi_warp_backward_matches_oracle(P, PW):
 
 def test_roi_warp_backward_null_outputs_and_limits():
     from mnc_b200 import ops
-    from mnc_b200._lib import lib, ptr, cur_stream, MncError, c_int, c_float
+    from mnc_b200._lib import lib, ptr, cur_stream, MncError
     feat, rois, top = _warp_case(7)
     f, r, t = _cuda(feat), _cuda(rois), _cuda(top)
     fd_only, none = ops.roi_warp_backward_nchw(f, r, t, 7, 7, want_rois=False)
@@ -58,8 +58,7 @@ def test_roi_warp_backward_null_outputs_and_limits():
     assert torch.equal(fd_only, fd) and torch.equal(rd_only, rd)
     # NULL rois_diff leaves nothing else written; R = 0 touches nothing
     sentinel = torch.full_like(f, 7.0)
-    rc = lib.mnc_roi_warp_backward_nchw(ptr(f), c_int(2), c_int(40), c_int(38), c_int(63), ptr(r),
-                                        c_int(0), c_int(7), c_int(7), c_float(0.0625), ptr(t),
+    rc = lib.mnc_roi_warp_backward_nchw(ptr(f), 2, 40, 38, 63, ptr(r), 0, 7, 7, 0.0625, ptr(t),
                                         ptr(sentinel), ptr(None), cur_stream())
     torch.cuda.synchronize()
     assert rc == 0 and bool((sentinel == 7.0).all())

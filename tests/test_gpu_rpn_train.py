@@ -213,16 +213,14 @@ def test_deterministic_and_graph_replay():
 
 def test_null_diffs_and_argument_errors():
     from mnc_b200 import ops
-    from mnc_b200._lib import MncError, lib, ptr, c_int, c_float
-    import ctypes
+    from mnc_b200._lib import MncError, lib, ptr
     f = fixture("A")
     c = config(f)
     out = _pt_device(f, True)
     st = out["state"]
-    assert lib.mnc_proposal_target_backward(ptr(out["rois"]), ptr(st), c_int(300), c_int(3), c_int(1),
-                                            ctypes.c_void_p(0), ctypes.c_void_p(0)) == 0
-    assert lib.mnc_proposal_backward(ptr(out["rois"]), c_int(0), ptr(st), ptr(out["rois"]), c_int(38),
-                                     c_int(63), c_float(0.0), ctypes.c_void_p(0), ctypes.c_void_p(0)) == 0
+    assert lib.mnc_proposal_target_backward(ptr(out["rois"]), ptr(st), 300, 3, 1, None, None) == 0
+    assert lib.mnc_proposal_backward(ptr(out["rois"]), 0, ptr(st), ptr(out["rois"]), 38, 63, 0.0,
+                                     None, None) == 0
     gt = _cuda(f["gt_boxes"])
     with pytest.raises(MncError):                  # G = 0
         ops.proposal_target(_cuda(f["rpn_rois"]), _cuda(f["rois_index"]), gt[:0],

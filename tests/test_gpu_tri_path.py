@@ -214,7 +214,7 @@ def test_softmax_rows_against_f64(rows, cols):
 
 def test_softmax_rows_default_output_and_arg_errors():
     from mnc_b200 import ops
-    from mnc_b200._lib import lib, ptr, cur_stream, c_int
+    from mnc_b200._lib import lib, ptr, cur_stream
     heads = torch.randn(9, 128, device="cuda")
     got = ops.softmax_rows(heads[:, 21:42], 21)
     assert got.shape == (9, 21) and got.is_contiguous()
@@ -222,7 +222,7 @@ def test_softmax_rows_default_output_and_arg_errors():
     assert float((got.double() - ref).abs().max()) < 1e-6
     out = torch.empty(9, 128, device="cuda")
     for cols in (0, 65):
-        rc = lib.mnc_softmax_rows(ptr(heads), c_int(128), c_int(9), c_int(cols), ptr(out), c_int(128), cur_stream())
+        rc = lib.mnc_softmax_rows(ptr(heads), 128, 9, cols, ptr(out), 128, cur_stream())
         assert rc == 1, "cols = %d: rc %d, expected MNC_ERR_ARG" % (cols, rc)
 
 
