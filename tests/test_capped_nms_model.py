@@ -19,14 +19,14 @@ def _iou_gt(a, b, thresh):
     return bool(inter / f(sa + sb - inter) > f(thresh))
 
 
-def capped_nms_blocks(boxes, thresh, max_keep, block):
+def capped_nms_blocks(n, suppresses, max_keep, block):
+    """suppresses(i, j): box i, earlier in score order, suppresses box j."""
     kept = []
-    n = len(boxes)
     for r0 in range(0, n, block):
         cand = range(r0, min(r0 + block, n))
         # phase A: suppression by earlier kept boxes + the block's own strictly upper triangle
-        sup = {c: any(_iou_gt(boxes[k], boxes[c], thresh) for k in kept) for c in cand}
-        diag = {i: {c for c in cand if c > i and _iou_gt(boxes[i], boxes[c], thresh)} for i in cand}
+        sup = {c: any(suppresses(k, c) for k in kept) for c in cand}
+        diag = {i: {c for c in cand if c > i and suppresses(i, c)} for i in cand}
         # phase B: serial resolve
         dead = {c for c in cand if sup[c]}
         for i in cand:
@@ -56,7 +56,7 @@ def test_block_walk_equals_greedy_nms(block, kind):
         boxes = util.random_boxes(n, seed=4)
     boxes = util.nudge_off_threshold(boxes, thresh)
     want = [int(i) for i in O.nms_sorted(boxes, thresh)[:max_keep]]
-    got = capped_nms_blocks(boxes, thresh, max_keep, block)
+    got = capped_nms_blocks(len(boxes), lambda i, j: _iou_gt(boxes[i], boxes[j], thresh), max_keep, block)
     assert got == want
     if kind == "clustered":
         assert len(want) == max_keep and want[-1] > 1.5 * max_keep    # suppression did happen
