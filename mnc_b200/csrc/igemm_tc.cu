@@ -68,25 +68,34 @@ constexpr int kSmemMax = 227 * 1024;   // opt-in shared memory of one sm_90 CTA
 
 // epilogue shared memory: the accumulator exchange (two 32-channel chunks of 128 rows, fp32, rows
 // padded to 33 words so that both the fragment writes and the row reads spread over the banks)
-// and the TMA-store staging (one buffer per consumer warpgroup x (hi, lo) x 128 rows x 64 B)
+// and the TMA-store staging (one buffer per consumer warpgroup x (hi, lo) x 128 rows x 64 B) share
+// one region: a chunk passes through the exchange before it is staged, so the exchange waits for
+// the previous chunk's stores to have read the staging instead of taking 33 KB of its own.  That
+// leaves the operand ring of conv tiles a third stage at BN = 128 (and a fourth at BN = 64).
 constexpr int kXchgStride = 33;
 constexpr int kXchgBytes = 2 * 128 * kXchgStride * 4;
 constexpr int kStagingBytes = 2 * 2 * 128 * 64;
+constexpr int kEpiBytes = kXchgBytes > kStagingBytes ? kXchgBytes : kStagingBytes;
 constexpr int kBarrierBytes = 1024;
 
 // A stage holds one 2-byte and one 2-byte (mode 0) or two 1-byte (mode 1) planes of the A tile
 // and of the B tile: the same bytes in both precision modes.
-template <int BN>
+template <int BN, int TH = 8>
 struct IgemmCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;  // one 2-byte plane of the A tile
   static constexpr int kBBytes = BN * kBlockK * 2;       // one 2-byte plane of the B tile
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-  static constexpr int kFixedBytes = 1024 /*align*/ + kBarrierBytes + kXchgBytes + kStagingBytes;
+  static constexpr int kFixedBytes = 1024 /*align*/ + kBarrierBytes + kEpiBytes;
   static constexpr int kStagesRaw = (kSmemMax - kFixedBytes) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
+  // the deeper ring pays for conv tiles only: measured on the H100, linear tiles (TH = 1) with a
+  // third / fourth stage made the whole step 6 % slower, so they run two / three
+  static constexpr int kCap = TH == 1 ? (BN == 128 ? 2 : 3) : 8;
+  static constexpr int kStages = kStagesRaw > kCap ? kCap : kStagesRaw;
   static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
   static_assert(kStages >= 2, "the ring needs two stages");
 };
+static_assert(IgemmCfg<128>::kStages == 3 && IgemmCfg<64>::kStages == 4,
+              "conv tiles run 3 operand stages at BN = 128 and 4 at BN = 64");
 
 struct Tile {
   int img, h0, w0, n0, ks;
@@ -145,9 +154,9 @@ struct EpiState {
 template <int TH, int TW, int BN>
 __device__ __forceinline__ void epilogue_tile(const IgemmArgs& p, const CUtensorMap* tm_o_hi_p,
                                               const CUtensorMap* tm_o_lo_p,
-                                              const CUtensorMap* tm_o_x_p, float* xchg,
-                                              uint8_t* staging, float (&acc)[BN / 64][32],
-                                              const Tile& tl, int grp, EpiState& st) {
+                                              const CUtensorMap* tm_o_x_p, uint8_t* staging,
+                                              float (&acc)[BN / 64][32], const Tile& tl, int grp,
+                                              EpiState& st) {
   const int tid = threadIdx.x & 127;
   const int lane = threadIdx.x & 31;
   constexpr int NBUF = 1;             // staging buffers per group
@@ -169,6 +178,12 @@ __device__ __forceinline__ void epilogue_tile(const IgemmArgs& p, const CUtensor
     const int c0 = nb * 64 + grp * 32;
     uint32_t r[32];
     {
+      float* xchg = reinterpret_cast<float*>(staging);
+      // the exchange overwrites the staging buffers: the previous chunk's stores must have read them
+      if (p.tma_store) {
+        if (threadIdx.x == lead) ptx::tma_store_wait_read<0>();
+        ptx::named_bar_sync(1, 256);
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int col = j * 8 + fcol;
@@ -295,8 +310,7 @@ __device__ __forceinline__ void epilogue_tile(const IgemmArgs& p, const CUtensor
         const bool tri = (p.out_mode == 4);
         const int buf = chunk_ctr % NBUF;
         uint8_t* sb = staging + (grp * NBUF + buf) * (2 * 128 * 64);
-        if (threadIdx.x == lead) ptx::tma_store_wait_read<NBUF - 1>();  // this buffer's previous store
-        ptx::named_bar_sync(3 + grp, 128);
+        // (the previous store from this buffer was waited for before the exchange)
         if (ch0 < p.Cout) {
           // bias: 8 x 16-byte loads when the chunk is whole and aligned (the usual case)
           float bv[32];
@@ -451,7 +465,7 @@ igemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
                 const __grid_constant__ CUtensorMap tm_o_x,
                 const IgemmArgs p) {
   static_assert(TH * TW == kBlockM, "pixel tile must have 128 rows");
-  using Cfg = IgemmCfg<BN>;
+  using Cfg = IgemmCfg<BN, TH>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kABytes = Cfg::kABytes;
   constexpr int kBBytes = Cfg::kBBytes;
@@ -463,7 +477,6 @@ igemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
   uint8_t* staging = smem + kStages * Cfg::kStageBytes + kBarrierBytes;  // 1024-aligned
-  float* xchg = reinterpret_cast<float*>(staging + kStagingBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -620,7 +633,7 @@ igemm_tc_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_consta
 #pragma unroll
           for (int j = 0; j < 32; ++j) acc[nb][j] += accc[nb][j];
       }
-      epilogue_tile<TH, TW, BN>(p, &tm_o_hi, &tm_o_lo, &tm_o_x, xchg, staging, acc, tl, grp, est);
+      epilogue_tile<TH, TW, BN>(p, &tm_o_hi, &tm_o_lo, &tm_o_x, staging, acc, tl, grp, est);
     }
     epilogue_finish(p, grp, est);
   }
@@ -642,7 +655,7 @@ constexpr int kC11ABytes = kBlockM * kC11K * 2; // one bf16 plane of the A tile:
 constexpr int kC11Stages = 2;
 constexpr int kC11BBytes = 128 * kC11K * 2;     // stacked weight tile: 8 KB
 constexpr int kC11Ring = kC11Stages * 2 * kC11ABytes + kC11BBytes;  // 40 KB
-constexpr int kC11Smem = kC11Ring + kBarrierBytes + kStagingBytes + kXchgBytes + 1024 /*align*/;
+constexpr int kC11Smem = kC11Ring + kBarrierBytes + kEpiBytes + 1024 /*align*/;
 constexpr int kC11Threads = 384;   // producer warpgroup + two consumer warpgroups
 
 __global__ void __launch_bounds__(kC11Threads, 1)
@@ -660,7 +673,6 @@ conv1_1_tc_kernel(const float* __restrict__ data, int B, int H, int W,
   uint64_t* a_empty = a_full + kC11Stages;
   uint64_t* b_full = a_empty + kC11Stages;
   uint8_t* staging = smem + kC11Ring + kBarrierBytes;
-  float* xchg = reinterpret_cast<float*>(staging + kStagingBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -771,7 +783,7 @@ conv1_1_tc_kernel(const float* __restrict__ data, int B, int H, int W,
         as = 0;
         aph ^= 1;
       }
-      epilogue_tile<1, 128, BN>(p, &tm_o_hi, &tm_o_lo, &tm_o_x, xchg, staging, acc, tl, grp, est);
+      epilogue_tile<1, 128, BN>(p, &tm_o_hi, &tm_o_lo, &tm_o_x, staging, acc, tl, grp, est);
     }
     epilogue_finish(p, grp, est);
   }
@@ -871,7 +883,7 @@ struct Maps {
 
 template <int TH, int TW, int BN, int PM>
 static int launch_igemm(const Maps& m, const IgemmArgs& a, int max_ctas, cudaStream_t stream) {
-  using Cfg = IgemmCfg<BN>;
+  using Cfg = IgemmCfg<BN, TH>;
   auto kern = igemm_tc_kernel<TH, TW, BN, PM>;
   static SmemGrant grant;
   if (!ensure_dynamic_smem(kern, Cfg::kSmemBytes, grant)) return MNC_ERR_CUDA;
