@@ -3,6 +3,7 @@ against the oracle's full aggregate: they must hold for every result, or the pru
 miss pixels."""
 import numpy as np
 
+from tests.mv_ties import rel_margin
 from tests.test_ref_pin import _voting_inputs
 
 
@@ -15,8 +16,8 @@ def _lists(boxes, scores):
 
 def test_covering_weight_region_contains_every_on_pixel():
     """mv_aggregate_kernel cuts the search region to the columns / rows whose covering weight
-    sum_i w_i [x in box_i] exceeds 0.4 (with the kernel's 1e-4 margin): valid because render <= 1
-    for masks in [0, 1] and weights >= 0.  Every pixel of {agg > 0.4} must lie inside."""
+    sum_i w_i [x in box_i] exceeds 0.4 (with the kernel's rounding margin, 1 + (n + 4) 2^-21):
+    valid because render <= 1 + 6 ulp for masks in [0, 1] and weights >= 0.  Every pixel of {agg > 0.4} must lie inside."""
     from oracle import oracle as O
     nb, H, W = 120, 150, 200
     rng = np.random.default_rng(5)
@@ -40,8 +41,9 @@ def test_covering_weight_region_contains_every_on_pixel():
             bx = boxes[i]
             ux += np.where(~((xs < bx[0]) | (xs > bx[2])), w, 0).astype(np.float32)
             uy += np.where(~((ys < bx[1]) | (ys > bx[3])), w, 0).astype(np.float32)
-        col_ok = ux * np.float32(1.0001) > np.float32(0.4)
-        row_ok = uy * np.float32(1.0001) > np.float32(0.4)
+        rel = rel_margin(len(ii))
+        col_ok = ux * rel > np.float32(0.4)
+        row_ok = uy * rel > np.float32(0.4)
         yy, xx = np.where(on)
         assert col_ok[xx].all() and row_ok[yy].all(), "result %d: an on pixel lies outside the pruned region" % t
         # and the tight box the oracle reports is the bounding box of the on pixels
