@@ -496,6 +496,52 @@ int mnc_anchor_target(int H, int W, int feat_stride, int allowed_border, const f
                       float* bbox_targets, float* bbox_inside_weights,
                       float* bbox_outside_weights, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Loss layers of the training net (SoftmaxWithLoss, SmoothL1Loss, SigmoidCrossEntropyLoss) and
+ * Accuracy, one image, fp32 device blobs in Caffe layout; stream-ordered, no host synchronisation,
+ * deterministic, no floating-point atomics (DESIGN.md "Loss layers").  Common arguments:
+ *   n_valid   device int, NULL: all rows.  Only the first *n_valid outer rows are real: rows past
+ *             it are not read, their diff (and prob) is written as 0, and every normaliser that
+ *             counts rows counts *n_valid (e.g. mnc_proposal_target's counts[0]).
+ *   top_diff  device float[1], the loss weight (Caffe's top[0]->cpu_diff()[0]).
+ *   loss      device float[1].  Loss sums are reduced in a fixed order in float64, rounded to
+ *             float32 once and divided by the normaliser in float32.
+ * Labels are float blobs read as static_cast<int>.
+ *
+ * mnc_softmax_loss: scores (outer, channels, inner), labels (outer, inner); normalization 0 FULL,
+ * 1 VALID, 2 BATCH_SIZE, 3 NONE (LossParameter.NormalizationMode); writes prob (outer, channels,
+ * inner), which mnc_softmax_loss_backward reads, and loss.  A label outside [0, channels) that is
+ * not the ignore label counts as valid, adds no loss term and no -1 to the diff.
+ * mnc_smooth_l1_loss: pred / target / inside_weights / outside_weights (num, dim), the weights both
+ * or neither (NULL); sigma as smooth_l1_loss_param.sigma; loss = sum / rows.  The backward writes
+ * the diff of pred only.
+ * mnc_sigmoid_ce_loss: x / targets / weights (num, dim), MNC's weighted form; weights NULL gives
+ * the two-bottom form (normaliser: rows).  With weights summing to 0 the loss is not written.
+ * mnc_accuracy: scores (outer, channels, inner), labels (outer, inner), 1 <= top_k <= channels;
+ * accuracy = hits / counted positions (0 / 0 is NaN, as in the reference). */
+int mnc_softmax_loss(const float* scores, const float* labels, int outer, int channels, int inner,
+                     const int* n_valid, int has_ignore, int ignore_label, int normalization,
+                     float* prob, float* loss, void* stream);
+int mnc_softmax_loss_backward(const float* prob, const float* labels, int outer, int channels,
+                              int inner, const int* n_valid, int has_ignore, int ignore_label,
+                              int normalization, const float* top_diff, float* bottom_diff,
+                              void* stream);
+int mnc_smooth_l1_loss(const float* pred, const float* target, const float* inside_weights,
+                       const float* outside_weights, int num, int dim, const int* n_valid,
+                       float sigma, float* loss, void* stream);
+int mnc_smooth_l1_loss_backward(const float* pred, const float* target,
+                                const float* inside_weights, const float* outside_weights, int num,
+                                int dim, const int* n_valid, float sigma, const float* top_diff,
+                                float* bottom_diff, void* stream);
+int mnc_sigmoid_ce_loss(const float* x, const float* targets, const float* weights, int num,
+                        int dim, const int* n_valid, float* loss, void* stream);
+int mnc_sigmoid_ce_loss_backward(const float* x, const float* targets, const float* weights,
+                                 int num, int dim, const int* n_valid, const float* top_diff,
+                                 float* bottom_diff, void* stream);
+int mnc_accuracy(const float* scores, const float* labels, int outer, int channels, int inner,
+                 const int* n_valid, int top_k, int has_ignore, int ignore_label, float* accuracy,
+                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -252,3 +252,78 @@ def anchor_target(H, W, gt_boxes, im_info, fg_inds=None, bg_inds=None, counts=No
     with torch.no_grad():
         return ops.anchor_target(H, W, gt_boxes.detach(), im_info.detach(), keys, fg_inds, bg_inds,
                                  counts, **kw)
+
+
+# ------------------------------------------------------------------ training-net loss layers
+class _SoftmaxLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, scores, labels, n_valid, ignore_label, normalization):
+        labels = _c(labels)
+        loss, prob = ops.softmax_loss(_c(scores), labels, ignore_label, normalization, n_valid)
+        ctx.save_for_backward(prob, labels, n_valid)
+        ctx.cfg = (ignore_label, normalization)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad):
+        prob, labels, n_valid = ctx.saved_tensors
+        g = ops.softmax_loss_backward(prob, labels, _c(grad), *ctx.cfg, n_valid=n_valid) \
+            if ctx.needs_input_grad[0] else None
+        return g, None, None, None, None
+
+
+class _SmoothL1Loss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pred, target, inside_weights, outside_weights, n_valid, sigma):
+        t = [None if v is None else _c(v) for v in (pred, target, inside_weights, outside_weights)]
+        ctx.save_for_backward(*t, n_valid)
+        ctx.sigma = sigma
+        return ops.smooth_l1_loss(*t, sigma=sigma, n_valid=n_valid)
+
+    @staticmethod
+    def backward(ctx, grad):
+        pred, target, wi, wo, n_valid = ctx.saved_tensors
+        g = ops.smooth_l1_loss_backward(pred, target, wi, wo, ctx.sigma, _c(grad), n_valid) \
+            if ctx.needs_input_grad[0] else None
+        return g, None, None, None, None, None
+
+
+class _SigmoidCELoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, targets, weights, n_valid):
+        t = [None if v is None else _c(v) for v in (x, targets, weights)]
+        ctx.save_for_backward(*t, n_valid)
+        return ops.sigmoid_ce_loss(*t, n_valid=n_valid)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, targets, weights, n_valid = ctx.saved_tensors
+        g = ops.sigmoid_ce_loss_backward(x, targets, weights, _c(grad), n_valid) \
+            if ctx.needs_input_grad[0] else None
+        return g, None, None, None
+
+
+def softmax_loss(scores, labels, n_valid=None, ignore_label=-1, normalization="VALID"):
+    """SoftmaxWithLoss (ops.softmax_loss): 0-d loss, differentiable in scores; the backward passes
+    grad_output as the loss weight.  Defaults: the training net's loss_param (ignore_label -1,
+    normalize true).  n_valid: int32 device count of the real rows (e.g. proposal_target's
+    counts[:1]) or None."""
+    return _SoftmaxLoss.apply(scores, labels, n_valid, ignore_label, normalization)
+
+
+def smooth_l1_loss(pred, target, inside_weights=None, outside_weights=None, sigma=1.0,
+                   n_valid=None):
+    """SmoothL1Loss (ops.smooth_l1_loss): 0-d loss = sum / rows, differentiable in pred."""
+    return _SmoothL1Loss.apply(pred, target, inside_weights, outside_weights, n_valid, sigma)
+
+
+def sigmoid_ce_loss(x, targets, weights=None, n_valid=None):
+    """SigmoidCrossEntropyLoss, MNC's weighted form (ops.sigmoid_ce_loss): 0-d loss,
+    differentiable in x; 0 when the weights sum to 0."""
+    return _SigmoidCELoss.apply(x, targets, weights, n_valid)
+
+
+def accuracy(scores, labels, top_k=1, ignore_label=None, n_valid=None):
+    """Accuracy (ops.accuracy); not differentiable.  The training net sets no ignore label."""
+    with torch.no_grad():
+        return ops.accuracy(scores.detach(), labels.detach(), top_k, ignore_label, n_valid)

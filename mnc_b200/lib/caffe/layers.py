@@ -177,3 +177,157 @@ class ROIPoolingLayer(_NativeLayer):
                                        bottom[0].shape, _dev(bottom[1].data).view(-1, 5),
                                        self.pooled_height_, self.pooled_width_, self.spatial_scale_)
         _diff(bottom[0])[...] = g.cpu().numpy()
+
+
+# ------------------------------------------------------------------ training-net loss layers
+class _LossLayer(_NativeLayer):
+    """LossLayer (loss_layer.cpp:8-27): loss_weight 1 unless given, which Layer::SetUp copies to
+    top[0]'s diff (layer.hpp:417-433); bottoms 0 and 1 agree in num; the top is a scalar."""
+
+    def LayerSetUp(self, bottom, top):
+        w = self.layer_param_.get("loss_weight", 1.0)
+        w = w[0] if isinstance(w, (list, tuple)) else w
+        top[0].diff = np.full((), w, dtype=np.float32)
+
+    def Reshape(self, bottom, top):
+        if bottom[0].num != bottom[1].num:
+            raise ValueError("The data and label should have the same number.")
+        top[0].reshape()
+
+    def _top_diff(self, top):
+        return _dev(top[0].diff)
+
+    def _no_label_backward(self, propagate_down):
+        if len(propagate_down) > 1 and any(propagate_down[1:]):
+            raise ValueError("%s Layer cannot backpropagate to label inputs." % self.TYPE)
+
+
+class SoftmaxWithLossLayer(_LossLayer):
+    """softmax_loss_layer.cpp:10-56 (setup / reshape), softmax_loss_layer.cu:32-124."""
+    TYPE = "SoftmaxWithLoss"
+
+    def LayerSetUp(self, bottom, top):
+        _LossLayer.LayerSetUp(self, bottom, top)
+        if self.layer_param_.get("softmax_param", {}).get("axis", 1) != 1:
+            raise ValueError("SoftmaxWithLoss: only the channel axis (1) is supported")
+        p = self.layer_param_.get("loss_param", {})
+        self.ignore_label_ = int(p["ignore_label"]) if "ignore_label" in p else None
+        if "normalization" not in p and "normalize" in p:
+            self.normalization_ = "VALID" if p["normalize"] else "BATCH_SIZE"
+        else:
+            self.normalization_ = p.get("normalization", "VALID")
+        if self.normalization_ not in ops.NORMALIZATION:
+            raise ValueError("Unknown normalization mode: %s" % self.normalization_)
+
+    def Reshape(self, bottom, top):
+        _LossLayer.Reshape(self, bottom, top)
+        b = bottom[0]
+        if b.num * (b.count // max(b.num * b.channels, 1)) != bottom[1].count:
+            raise ValueError("Number of labels must match number of predictions")
+        if len(top) >= 2:
+            top[1].reshape(*b.shape)
+
+    def Forward_gpu(self, bottom, top):
+        loss, self.prob_ = ops.softmax_loss(_dev(bottom[0].data), _dev(bottom[1].data),
+                                            self.ignore_label_, self.normalization_)
+        top[0].data[...] = loss.cpu().numpy()
+        if len(top) == 2:
+            top[1].data[...] = self.prob_.cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        self._no_label_backward(propagate_down)
+        if propagate_down[0]:
+            g = ops.softmax_loss_backward(self.prob_, _dev(bottom[1].data), self._top_diff(top),
+                                          self.ignore_label_, self.normalization_)
+            _diff(bottom[0])[...] = g.cpu().numpy()
+
+
+class SmoothL1LossLayer(_LossLayer):
+    """smooth_L1_loss_layer.cpp:13-44 (setup / reshape), smooth_L1_loss_layer.cu:31-106.  The
+    backward to bottom 1 (the targets) is not reachable in the training net and not provided."""
+    TYPE = "SmoothL1Loss"
+
+    def LayerSetUp(self, bottom, top):
+        _LossLayer.LayerSetUp(self, bottom, top)
+        self.sigma_ = float(self.layer_param_.get("smooth_l1_loss_param", {}).get("sigma", 1.0))
+        self.has_weights_ = len(bottom) >= 3
+        if self.has_weights_ and len(bottom) != 4:
+            raise ValueError("If weights are used, must specify both inside and outside weights")
+
+    def Reshape(self, bottom, top):
+        _LossLayer.Reshape(self, bottom, top)
+        b = bottom[0]
+        for o in bottom[1:]:
+            if (o.channels, o.height, o.width) != (b.channels, b.height, b.width):
+                raise ValueError("SmoothL1Loss: bottoms must agree in channels, height and width")
+
+    def _args(self, bottom):
+        t = [_dev(x.data) for x in bottom]
+        return t + [None] * (4 - len(t))
+
+    def Forward_gpu(self, bottom, top):
+        top[0].data[...] = ops.smooth_l1_loss(*self._args(bottom), sigma=self.sigma_).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        if len(propagate_down) > 1 and propagate_down[1]:
+            raise ValueError("SmoothL1Loss: the backward to the targets is not provided")
+        if propagate_down[0]:
+            g = ops.smooth_l1_loss_backward(*self._args(bottom), sigma=self.sigma_,
+                                            top_diff=self._top_diff(top))
+            _diff(bottom[0])[...] = g.cpu().numpy()
+
+
+class SigmoidCrossEntropyLossLayer(_LossLayer):
+    """sigmoid_cross_entropy_loss_layer.cpp:8-97, MNC's form: a third bottom weighs each element
+    and normalises by the weights' sum; with that sum 0 the top is left as it was."""
+    TYPE = "SigmoidCrossEntropyLoss"
+
+    def Reshape(self, bottom, top):
+        _LossLayer.Reshape(self, bottom, top)
+        if bottom[0].count != bottom[1].count:
+            raise ValueError("SIGMOID_CROSS_ENTROPY_LOSS layer inputs must have the same count.")
+        if len(bottom) == 3 and bottom[0].count != bottom[2].count:
+            raise ValueError("SIGMOID_CROSS_ENTROPY_LOSS layer weight must be the same count")
+
+    def _args(self, bottom):
+        return [_dev(x.data) for x in bottom[:3]] + [None] * (3 - min(len(bottom), 3))
+
+    def Forward_gpu(self, bottom, top):
+        out = _dev(top[0].data if top[0].data.shape == () else 0.0).reshape(())
+        top[0].data[...] = ops.sigmoid_ce_loss(*self._args(bottom), out=out).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        self._no_label_backward(propagate_down)
+        if propagate_down[0]:
+            g = ops.sigmoid_ce_loss_backward(*self._args(bottom), top_diff=self._top_diff(top))
+            _diff(bottom[0])[...] = g.cpu().numpy()
+
+
+class AccuracyLayer(_NativeLayer):
+    """accuracy_layer.cpp:10-103, top 0 only (the per-class top is not provided)."""
+
+    def LayerSetUp(self, bottom, top):
+        p = self.layer_param_.get("accuracy_param", {})
+        self.top_k_ = int(p.get("top_k", 1))
+        self.ignore_label_ = int(p["ignore_label"]) if "ignore_label" in p else None
+        if p.get("axis", 1) != 1:
+            raise ValueError("Accuracy: only the channel axis (1) is supported")
+        if len(top) > 1:
+            raise ValueError("Accuracy: the per-class top is not provided")
+
+    def Reshape(self, bottom, top):
+        b = bottom[0]
+        if self.top_k_ > b.count // max(bottom[1].count, 1):
+            raise ValueError("top_k must be less than or equal to the number of classes.")
+        if b.num * (b.count // max(b.num * b.channels, 1)) != bottom[1].count:
+            raise ValueError("Number of labels must match number of predictions")
+        top[0].reshape()
+
+    def Forward_gpu(self, bottom, top):
+        top[0].data[...] = ops.accuracy(_dev(bottom[0].data), _dev(bottom[1].data), self.top_k_,
+                                        self.ignore_label_).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        if any(propagate_down):
+            raise NotImplementedError("NOT_IMPLEMENTED (as in the reference)")
+

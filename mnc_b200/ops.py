@@ -749,3 +749,144 @@ def anchor_target(H, W, gt_boxes, im_info, keys, fg_inds=None, bg_inds=None, cou
         (ctypes.c_float * 4)(*[float(x) for x in inside_weights]), ptr(ws), ptr(labels),
         ptr(t[0]), ptr(t[1]), ptr(t[2]), cur_stream()), "mnc_anchor_target", launches=5)
     return (labels, *t)
+
+
+# ------------------------------------------------------------------ training-net loss layers
+NORMALIZATION = {"FULL": 0, "VALID": 1, "BATCH_SIZE": 2, "NONE": 3}
+
+
+def _nv(n_valid):
+    """n_valid as an int32 device count (None: all rows)."""
+    return None if n_valid is None else n_valid.reshape(-1)[:1].contiguous().to(torch.int32)
+
+
+def _loss_weight(top_diff, dev):
+    if top_diff is None:
+        return torch.ones((), dtype=torch.float32, device=dev)
+    return _f32(top_diff).reshape(())
+
+
+def _onc(x, label_count):
+    """(outer, channels, inner) of a softmax / accuracy bottom along axis 1."""
+    outer = x.shape[0]
+    C = x.shape[1] if x.dim() > 1 else 1
+    inner = x.numel() // max(outer * C, 1)
+    if outer * inner != label_count:
+        raise ValueError("number of labels must match number of predictions")
+    return outer, C, inner
+
+
+def softmax_loss(scores, labels, ignore_label=None, normalization="VALID", n_valid=None):
+    """SoftmaxWithLoss forward (softmax_loss_layer.cu:32-68) over axis 1 of scores (outer, C, ...),
+    labels (outer, ...) as floats.  n_valid: int32 device count of the real outer rows, or None.
+    -> (loss 0-d, prob like scores)."""
+    scores = _f32(scores)
+    outer, C, inner = _onc(scores, labels.numel())
+    labels, n_valid = _f32(labels), _nv(n_valid)     # held until the call returns
+    prob = torch.empty_like(scores)
+    loss = torch.zeros((), dtype=torch.float32, device=scores.device)
+    check(lib.mnc_softmax_loss(ptr(scores), ptr(labels), outer, C, inner, ptr(n_valid),
+                               int(ignore_label is not None), int(ignore_label or 0),
+                               NORMALIZATION[normalization], ptr(prob), ptr(loss), cur_stream()),
+          "mnc_softmax_loss")
+    return loss, prob
+
+
+def softmax_loss_backward(prob, labels, top_diff=None, ignore_label=None, normalization="VALID",
+                          n_valid=None):
+    """SoftmaxWithLoss backward (softmax_loss_layer.cu:70-124): -> the scores' diff."""
+    prob = _f32(prob)
+    outer, C, inner = _onc(prob, labels.numel())
+    labels, n_valid, top_diff = _f32(labels), _nv(n_valid), _loss_weight(top_diff, prob.device)
+    out = torch.empty_like(prob)
+    check(lib.mnc_softmax_loss_backward(ptr(prob), ptr(labels), outer, C, inner,
+                                        ptr(n_valid), int(ignore_label is not None),
+                                        int(ignore_label or 0), NORMALIZATION[normalization],
+                                        ptr(top_diff), ptr(out),
+                                        cur_stream()), "mnc_softmax_loss_backward")
+    return out
+
+
+def _nd(x, *others):
+    num = x.shape[0]
+    dim = x.numel() // max(num, 1)
+    for o in others:
+        if o is not None and o.numel() != x.numel():
+            raise ValueError("loss bottoms must have the same count")
+    return num, dim
+
+
+def _weights(inside_weights, outside_weights):
+    if (inside_weights is None) != (outside_weights is None):
+        raise ValueError("If weights are used, must specify both inside and outside weights")
+    return (None, None) if inside_weights is None else (_f32(inside_weights), _f32(outside_weights))
+
+
+def smooth_l1_loss(pred, target, inside_weights=None, outside_weights=None, sigma=1.0,
+                   n_valid=None):
+    """SmoothL1Loss forward (smooth_L1_loss_layer.cu:31-63): -> loss 0-d = sum / rows."""
+    pred = _f32(pred)
+    num, dim = _nd(pred, target, inside_weights, outside_weights)
+    wi, wo = _weights(inside_weights, outside_weights)
+    target, n_valid = _f32(target), _nv(n_valid)
+    loss = torch.zeros((), dtype=torch.float32, device=pred.device)
+    check(lib.mnc_smooth_l1_loss(ptr(pred), ptr(target), ptr(wi), ptr(wo), num, dim,
+                                 ptr(n_valid), sigma, ptr(loss), cur_stream()),
+          "mnc_smooth_l1_loss")
+    return loss
+
+
+def smooth_l1_loss_backward(pred, target, inside_weights=None, outside_weights=None, sigma=1.0,
+                            top_diff=None, n_valid=None):
+    """SmoothL1Loss backward to bottom 0 (smooth_L1_loss_layer.cu:67-106): -> pred's diff."""
+    pred = _f32(pred)
+    num, dim = _nd(pred, target, inside_weights, outside_weights)
+    wi, wo = _weights(inside_weights, outside_weights)
+    target, n_valid, top_diff = _f32(target), _nv(n_valid), _loss_weight(top_diff, pred.device)
+    out = torch.empty_like(pred)
+    check(lib.mnc_smooth_l1_loss_backward(ptr(pred), ptr(target), ptr(wi), ptr(wo), num, dim,
+                                          ptr(n_valid), sigma, ptr(top_diff), ptr(out),
+                                          cur_stream()), "mnc_smooth_l1_loss_backward")
+    return out
+
+
+def sigmoid_ce_loss(x, targets, weights=None, n_valid=None, out=None):
+    """SigmoidCrossEntropyLoss forward, MNC's form (sigmoid_cross_entropy_loss_layer.cpp:31-59):
+    -> loss 0-d.  When the weights sum to 0 the reference leaves the top as it was: the result is
+    then `out` unchanged (a float32 0-d device tensor) or 0 without it."""
+    x = _f32(x)
+    num, dim = _nd(x, targets, weights)
+    targets, n_valid = _f32(targets), _nv(n_valid)
+    weights = None if weights is None else _f32(weights)
+    loss = torch.zeros((), dtype=torch.float32, device=x.device) if out is None else out
+    check(lib.mnc_sigmoid_ce_loss(ptr(x), ptr(targets), ptr(weights), num, dim, ptr(n_valid),
+                                  ptr(loss), cur_stream()),
+          "mnc_sigmoid_ce_loss")
+    return loss
+
+
+def sigmoid_ce_loss_backward(x, targets, weights=None, top_diff=None, n_valid=None):
+    """SigmoidCrossEntropyLoss backward (sigmoid_cross_entropy_loss_layer.cpp:62-92): -> x's diff."""
+    x = _f32(x)
+    num, dim = _nd(x, targets, weights)
+    targets, n_valid, top_diff = _f32(targets), _nv(n_valid), _loss_weight(top_diff, x.device)
+    weights = None if weights is None else _f32(weights)
+    out = torch.empty_like(x)
+    check(lib.mnc_sigmoid_ce_loss_backward(ptr(x), ptr(targets), ptr(weights), num, dim,
+                                           ptr(n_valid), ptr(top_diff), ptr(out),
+                                           cur_stream()), "mnc_sigmoid_ce_loss_backward")
+    return out
+
+
+def accuracy(scores, labels, top_k=1, ignore_label=None, n_valid=None):
+    """Accuracy forward (accuracy_layer.cpp:48-103) over axis 1: -> 0-d fraction of hits."""
+    scores = _f32(scores)
+    outer, C, inner = _onc(scores, labels.numel())
+    if not 1 <= top_k <= C:
+        raise ValueError("top_k must be less than or equal to the number of classes")
+    labels, n_valid = _f32(labels), _nv(n_valid)
+    out = torch.empty((), dtype=torch.float32, device=scores.device)
+    check(lib.mnc_accuracy(ptr(scores), ptr(labels), outer, C, inner, ptr(n_valid),
+                           top_k, int(ignore_label is not None), int(ignore_label or 0), ptr(out),
+                           cur_stream()), "mnc_accuracy")
+    return out
