@@ -268,6 +268,8 @@ int mnc_bbox_overlaps_host(const double* boxes, int N, const double* query, int 
  * after per-class rank sort + NMS (mnc_rank_sort_desc / mnc_gather_boxes / mnc_nms_sorted with
  * problems = batch*(ncls-1)), vote_select picks the global threshold and enumerates results,
  * vote_candidates builds the (inds, weights) lists, mv_device renders/aggregates/resizes.
+ * vote_select keeps its (ncls-1)*max_per_image entries in the 48 KB of shared memory a launch
+ * gets without an opt-in, or returns MNC_ERR_ARG (21 classes: max_per_image <= 199).
  * mv_device's bbox_ws: int32 workspace of batch*max_results*4 + batch entries. */
 int mnc_vote_select(const float* scores, int nb, int ncls, const int* order, const int* keep,
                     int keep_stride, const int* num_keep, int max_per_image, int max_results,

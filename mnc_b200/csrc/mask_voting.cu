@@ -691,7 +691,14 @@ extern "C" int mnc_vote_select(const float* scores, int nb, int ncls, const int*
                                int* overflow, void* stream_) {
   const int cap = (ncls - 1) * max_per_image;
   const int smem = cap * 12 + (ncls + 1) * 4;
-  if (smem > 48 * 1024) return MNC_ERR_ARG;
+  // without an opt-in, the kernel's static shared memory and the dynamic part share 48 KB
+  static const int static_smem = [] {
+    cudaFuncAttributes a{};
+    return cudaFuncGetAttributes(&a, vote_select_kernel) == cudaSuccess
+               ? static_cast<int>(a.sharedSizeBytes) : -1;
+  }();
+  if (static_smem < 0) return MNC_ERR_CUDA;
+  if (smem + static_smem > 48 * 1024) return MNC_ERR_ARG;
   vote_select_kernel<<<batch, 1024, smem, static_cast<cudaStream_t>(stream_)>>>(
       scores, nb, ncls, order, keep, keep_stride, num_keep, max_per_image, max_results,
       res_box_idx, res_class, res_score, n_res, class_bar, overflow);

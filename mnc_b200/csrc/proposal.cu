@@ -50,7 +50,12 @@ static void generate_anchors_host(double out[9][4]) {
   }
 }
 
-__device__ __forceinline__ float clipf(float v, float hi) { return fmaxf(fminf(v, hi), 0.f); }
+// np.maximum(np.minimum(v, hi), 0) of clip_boxes: a NaN coordinate stays NaN (fminf / fmaxf
+// would return the other operand).  rpn_decode's min-size test is false for a NaN side, so such a
+// proposal is dropped as in filter_small_boxes.
+__device__ __forceinline__ float clipf(float v, float hi) {
+  return v != v ? v : fmaxf(fminf(v, hi), 0.f);
+}
 
 // bbox_transform_inv (bbox_decode.cuh), then clip_boxes (bbox_transform.py:112-118).
 __device__ __forceinline__ void decode_clip(float x1, float y1, float x2, float y2, float dx,
