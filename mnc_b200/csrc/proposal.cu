@@ -145,7 +145,8 @@ __global__ void write_rois_kernel(const float* __restrict__ sorted_boxes, int n_
 }
 
 // One thread per RoI: c* = first argmax over all `ncls` seg_cls_prob columns (bg allowed),
-// decode the 4 deltas of class c*, clip to im_info (stage_bridge_layer.py:241-252).
+// decode the 4 deltas of class c*, clip to im_info (stage_bridge_layer.py:241-252).  As numpy's
+// argmax, the first NaN of a row wins over any number: once bv is NaN no later column replaces it.
 __global__ void stage_bridge_kernel(const float* __restrict__ rois,
                                     const float* __restrict__ bbox_pred, int bbox_stride,
                                     const float* __restrict__ seg_cls_prob, int prob_stride,
@@ -160,7 +161,7 @@ __global__ void stage_bridge_kernel(const float* __restrict__ rois,
   float bv = p[0];
   for (int c = 1; c < ncls; ++c) {
     const float v = p[c];
-    if (v > bv) {
+    if (v > bv || (v != v && bv == bv)) {
       bv = v;
       best = c;
     }
