@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import roi_shapes as RS
 from tests import util
 
 pytestmark = pytest.mark.gpu
@@ -23,18 +24,30 @@ def _rois(n, seed, W=1000, H=600, extra=True):
     return rois.astype(np.float32)
 
 
-@pytest.mark.parametrize("P", [28, 14, 7])
-def test_roi_warp_nchw_bit_exact(P):
+def table_params(pool_only=False):
+    """(case, size) parameters, size = (ph, pw), over the shape table of tests/roi_shapes.py."""
+    return [pytest.param(n, (ph, pw), id=RS.size_id(n, ph, pw)) for n, ph, pw in RS.sizes(pool_only)]
+
+
+@pytest.mark.parametrize("case,size", [pytest.param(None, (P, P), id=str(P)) for P in (28, 14, 7)] + table_params())
+def test_roi_warp_nchw_bit_exact(case, size):
     from oracle import oracle as O
     from mnc_b200 import ops
-    rng = np.random.default_rng(7)
-    feat = np.maximum(rng.normal(size=(2, 40, 38, 63)), 0).astype(np.float32)
-    rois = _rois(64, 8)
-    rois[10:20, 0] = 1  # second image of the batch (roi_warping_layer.cu:79,96)
-    want = O.roi_warp(feat, rois, P, P)
-    got = ops.roi_warp_nchw(torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda(), P, P).cpu().numpy()
+    ph, pw = size
+    if case is None:
+        rng = np.random.default_rng(7)
+        feat = np.maximum(rng.normal(size=(2, 40, 38, 63)), 0).astype(np.float32)
+        rois = _rois(64, 8)
+        rois[10:20, 0] = 1  # second image of the batch (roi_warping_layer.cu:79,96)
+        ss = 0.0625
+    else:
+        feat, rois, ss = RS.feat(case), RS.rois(case), RS.BY_NAME[case].scale
+    want = O.roi_warp(feat, rois, ph, pw, ss)
+    got = ops.roi_warp_nchw(torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda(), ph, pw, ss).cpu().numpy()
     assert np.array_equal(got, want)
-    assert np.abs(want[3]).max() == 0.0
+    for r in ([3] if case is None else RS.outside_rows(case)):
+        assert np.abs(want[r]).max() == 0.0
+    assert np.abs(want).max() > 0
 
 
 def test_roi_warp_layer_mirror_contract():
@@ -82,6 +95,19 @@ def test_mask_resize_and_pool_bit_exact():
                           O.mask_pool(f2, k2))
     with pytest.raises(ValueError):
         ops.mask_pool_nchw(torch.from_numpy(f2).cuda(), torch.from_numpy(k2[:, :, :6]).contiguous().cuda())
+    # a blob larger than one grid-stride pass, through the vector kernel and, offset by one float
+    # (a view: 4-byte aligned only), through the scalar one
+    shape = RS.MASK_POOL["pool_64x512"]
+    f3 = rng.normal(size=shape).astype(np.float32)
+    k3 = rng.uniform(size=(shape[0], 1) + shape[2:]).astype(np.float32)
+    want = O.mask_pool(f3, k3)
+    d_k3 = torch.from_numpy(k3).cuda()
+    assert np.array_equal(ops.mask_pool_nchw(torch.from_numpy(f3).cuda(), d_k3).cpu().numpy(), want)
+    store = torch.empty(f3.size + 1, device="cuda")
+    d_f3 = store[1:].view(shape)
+    d_f3.copy_(torch.from_numpy(f3))
+    assert d_f3.data_ptr() % 16 == 4
+    assert np.array_equal(ops.mask_pool_nchw(d_f3, d_k3).cpu().numpy(), want)
 
 
 @pytest.mark.parametrize("sub", [2, 1])

@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_roi import _rois
+from tests import roi_shapes as RS
+from tests.test_gpu_roi import _rois, table_params
 
 pytestmark = pytest.mark.gpu
 
@@ -25,24 +26,50 @@ def _warp_case(P, PW=None, seed=0):
     return feat, rois, top
 
 
-@pytest.mark.parametrize("P,PW", [(28, 28), (14, 14), (7, 7), (9, 5)])
-def test_roi_warp_backward_matches_oracle(P, PW):
+def _table_case(case, ph, pw):
+    """feat, rois, top_diff and spatial scale of a case of tests/roi_shapes.py."""
+    return RS.feat(case), RS.rois(case), RS.top_diff(case, ph, pw), RS.BY_NAME[case].scale
+
+
+def _images_without_rois(feat, rois):
+    return sorted(set(range(feat.shape[0])) - set(rois[:, 0].astype(int).tolist()))
+
+
+def _same_bits(a, b):
+    return np.array_equal(np.asarray(a).view(np.uint32), np.asarray(b).view(np.uint32))
+
+
+@pytest.mark.parametrize("case,size", [pytest.param(None, (P, PW), id="%d-%d" % (P, PW))
+                                       for P, PW in [(28, 28), (14, 14), (7, 7), (9, 5)]] + table_params())
+def test_roi_warp_backward_matches_oracle(case, size):
     from oracle import oracle_backward as OB
     from mnc_b200 import ops
-    feat, rois, top = _warp_case(P, PW)
-    want_f, want_r, mag = OB.roi_warp_backward(feat, rois, top, P, PW, want_abs=True)
-    fd, rd = ops.roi_warp_backward_nchw(_cuda(feat), _cuda(rois), _cuda(top), P, PW)
+    P, PW = size
+    if case is None:
+        feat, rois, top = _warp_case(P, PW)
+        ss = 0.0625
+    else:
+        feat, rois, top, ss = _table_case(case, P, PW)
+    want_f, want_r, mag = OB.roi_warp_backward(feat, rois, top, P, PW, ss, want_abs=True)
+    fd, rd = ops.roi_warp_backward_nchw(_cuda(feat), _cuda(rois), _cuda(top), P, PW, ss)
     fd, rd = fd.cpu().numpy(), rd.cpu().numpy()
     assert np.array_equal(fd, want_f)
     assert np.abs(want_f).max() > 0
     assert np.all(rd[:, 0] == 0)
     assert np.all(np.abs(rd - want_r) <= 1e-5 * mag + 1e-30)
-    assert np.abs(want_r).max() > 0
+    H, W = feat.shape[2:]
+    if H > 1 and W > 1:
+        # (on a single row or column every sample's second tap lies past the map: no term)
+        assert np.abs(want_r).max() > 0
     # RoI 3 lies entirely outside the map: every sample is out of range and contributes 0
-    assert np.all(rd[3] == 0)
+    for r in ([3] if case is None else RS.outside_rows(case)):
+        assert np.all(rd[r] == 0)
+    # an image no RoI points at gets exact +0.0 (the output comes from torch.empty)
+    for n in _images_without_rois(feat, rois):
+        assert _same_bits(fd[n], np.zeros_like(fd[n]))
     # a second call gives the same bits
-    fd2, rd2 = ops.roi_warp_backward_nchw(_cuda(feat), _cuda(rois), _cuda(top), P, PW)
-    assert np.array_equal(fd2.cpu().numpy(), fd) and np.array_equal(rd2.cpu().numpy(), rd)
+    fd2, rd2 = ops.roi_warp_backward_nchw(_cuda(feat), _cuda(rois), _cuda(top), P, PW, ss)
+    assert _same_bits(fd2.cpu().numpy(), fd) and _same_bits(rd2.cpu().numpy(), rd)
 
 
 def test_roi_warp_backward_null_outputs_and_limits():
@@ -70,18 +97,21 @@ def test_roi_warp_backward_null_outputs_and_limits():
     assert not z[0].any() and z[1].shape == (0, 5)
 
 
-@pytest.mark.parametrize("oh,ow", [(14, 14), (7, 9), (21, 21), (28, 28)])
-def test_mask_resize_backward_matches_oracle(oh, ow):
+@pytest.mark.parametrize("oh,ow,planes", [pytest.param(oh, ow, (37, 2), id="%d-%d" % (oh, ow))
+                                           for oh, ow in [(14, 14), (7, 9), (21, 21), (28, 28)]] +
+                         [pytest.param(o[0], o[1], s[:2], id=k) for k, (s, o) in RS.MASK_RESIZE_BWD.items()])
+def test_mask_resize_backward_matches_oracle(oh, ow, planes):
     from oracle import oracle_backward as OB
     from mnc_b200 import ops
     rng = np.random.default_rng(oh + ow)
-    g = rng.normal(size=(37, 2, oh, ow)).astype(np.float32)
+    g = rng.normal(size=planes + (oh, ow)).astype(np.float32)
     got = ops.mask_resize_backward_nchw(_cuda(g), 21, 21).cpu().numpy()
     want = OB.mask_resize_backward(g, 21, 21)
     assert np.array_equal(got, want) and np.abs(want).max() > 0
 
 
-@pytest.mark.parametrize("shape", [(64, 24, 14, 14), (3, 5, 7, 9)])
+@pytest.mark.parametrize("shape", [pytest.param(s, id="shape%d" % i) for i, s in enumerate([(64, 24, 14, 14), (3, 5, 7, 9)])] +
+                         [pytest.param(s, id=k) for k, s in RS.MASK_POOL.items()])
 def test_mask_pool_backward_matches_oracle(shape):
     from oracle import oracle_backward as OB
     from mnc_b200 import ops
@@ -97,20 +127,26 @@ def test_mask_pool_backward_matches_oracle(shape):
     assert none is None and torch.equal(md2, md)
 
 
-@pytest.mark.parametrize("P", [7, 14])
-def test_roi_pool_backward_matches_oracle(P):
+@pytest.mark.parametrize("case,size", [pytest.param(None, (P, P), id=str(P)) for P in (7, 14)] + table_params())
+def test_roi_pool_backward_matches_oracle(case, size):
     from oracle import oracle_backward as OB
     from mnc_b200 import ops
-    feat, rois, _ = _warp_case(P, seed=3)
-    rng = np.random.default_rng(P)
-    arg = torch.empty((rois.shape[0], 40, P, P), dtype=torch.int32, device="cuda")
-    ops.roi_pool_nchw(_cuda(feat), _cuda(rois), P, P, argmax=arg)
-    g = rng.normal(size=(rois.shape[0], 40, P, P)).astype(np.float32)
-    want = OB.roi_pool_backward(g, arg.cpu().numpy(), feat.shape, rois, P, P)
-    got = ops.roi_pool_backward_nchw(_cuda(g), arg, feat.shape, _cuda(rois), P, P)
+    P, PW = size
+    if case is None:
+        feat, rois, _ = _warp_case(P, seed=3)
+        g = np.random.default_rng(P).normal(size=(rois.shape[0], 40, P, P)).astype(np.float32)
+        ss = 0.0625
+    else:
+        feat, rois, g, ss = _table_case(case, P, PW)
+    arg = torch.empty(g.shape, dtype=torch.int32, device="cuda")
+    ops.roi_pool_nchw(_cuda(feat), _cuda(rois), P, PW, ss, argmax=arg)
+    want = OB.roi_pool_backward(g, arg.cpu().numpy(), feat.shape, rois, P, PW, ss)
+    got = ops.roi_pool_backward_nchw(_cuda(g), arg, feat.shape, _cuda(rois), P, PW, ss)
     assert np.array_equal(got.cpu().numpy(), want) and np.abs(want).max() > 0
-    again = ops.roi_pool_backward_nchw(_cuda(g), arg, feat.shape, _cuda(rois), P, P)
-    assert torch.equal(again, got)
+    for n in _images_without_rois(feat, rois):
+        assert _same_bits(got[n].cpu().numpy(), np.zeros_like(want[n]))
+    again = ops.roi_pool_backward_nchw(_cuda(g), arg, feat.shape, _cuda(rois), P, PW, ss)
+    assert _same_bits(again.cpu().numpy(), got.cpu().numpy())
 
 
 def test_layer_mirrors_backward():

@@ -5,7 +5,9 @@ import numpy as np
 import pytest
 import torch
 
+from tests import roi_shapes as RS
 from tests import util
+from tests.test_gpu_roi import table_params
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -24,21 +26,33 @@ def _rois(n, seed, W, H, levels=1):
     return r
 
 
-@pytest.mark.parametrize("P", [7, 14, (6, 3)])
-def test_roi_pool_nchw_bit_exact(P):
+@pytest.mark.parametrize("case,size", [pytest.param(None, (P, P), id=str(P)) for P in (7, 14)] +
+                         [pytest.param(None, (6, 3), id="P2")] + table_params(pool_only=True))
+def test_roi_pool_nchw_bit_exact(case, size):
     from oracle import oracle as O
     from mnc_b200 import ops
-    ph, pw = (P, P) if isinstance(P, int) else P
-    rng = np.random.default_rng(5)
-    feat = rng.normal(size=(2, 40, 38, 63)).astype(np.float32)
-    rois = _rois(64, 6, 1000, 600, levels=2)
-    want, want_arg = O.roi_pool(feat, rois, ph, pw, return_argmax=True)
+    from mnc_b200._lib import MncError
+    ph, pw = size
+    if case is None:
+        rng = np.random.default_rng(5)
+        feat = rng.normal(size=(2, 40, 38, 63)).astype(np.float32)
+        rois = _rois(64, 6, 1000, 600, levels=2)
+        ss = 0.0625
+    else:
+        feat, rois, ss = RS.feat(case), RS.rois(case), RS.BY_NAME[case].scale
+    want, want_arg = O.roi_pool(feat, rois, ph, pw, ss, return_argmax=True)
     d_feat, d_rois = torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda()
-    arg = torch.empty((64, 40, ph, pw), dtype=torch.int32, device="cuda")
-    got = ops.roi_pool_nchw(d_feat, d_rois, ph, pw, argmax=arg)
+    arg = torch.empty(want.shape, dtype=torch.int32, device="cuda")
+    got = ops.roi_pool_nchw(d_feat, d_rois, ph, pw, ss, argmax=arg)
     assert np.array_equal(got.cpu().numpy(), want)
     assert np.array_equal(arg.cpu().numpy(), want_arg)
-    assert np.array_equal(ops.roi_pool_nchw(d_feat, d_rois, ph, pw).cpu().numpy(), want)  # argmax=NULL
+    assert np.array_equal(ops.roi_pool_nchw(d_feat, d_rois, ph, pw, ss).cpu().numpy(), want)  # argmax=NULL
+    assert (want_arg >= 0).any()
+    if max(ph, pw) > 32:
+        # the forward takes any size whose bins fit in shared memory; the backward stages per-RoI
+        # tables of at most 32 cells a side and rejects larger ones
+        with pytest.raises(MncError):
+            ops.roi_pool_backward_nchw(got, arg, feat.shape, d_rois, ph, pw, ss)
 
 
 def test_roi_pooling_layer_mirror_contract():
@@ -62,24 +76,36 @@ def test_roi_pooling_layer_mirror_contract():
         ROIPoolingLayer(dict(roi_pooling_param=dict(pooled_w=7, pooled_h=0))).LayerSetUp([feat, rois], [top])
 
 
-@pytest.mark.parametrize("P", [7, 14])
-def test_roi_pool_and_sample_split_forms(P):
-    """Engine forms (fp32 NHWC in, split-bf16 rows out) vs the NCHW layer kernels' oracle."""
+@pytest.mark.parametrize("C,P", [pytest.param(64, P, id=str(P)) for P in (7, 14)] +
+                         [pytest.param(C, P, id="C%d-P%d" % (C, P)) for C in (4, 12, 512) for P in (1, 7, 14, 32)])
+def test_roi_pool_and_sample_split_forms(C, P):
+    """Engine forms (fp32 NHWC in, split-bf16 rows [r][ph][pw][c] out) vs the NCHW layer kernels'
+    oracle.  ROIPooling is a max, so its rows are the split of the oracle's bytes exactly.
+    ROIWarping is evaluated with FMAs: per element |got - want| <= 2^-16 |want| + 2^-20 S, with
+    S = sum_i w_i |v_i| = roi_warp(|feat|) (the weights are non-negative) -- twice the split
+    rounding plus twice the fused-versus-unfused difference of the 4-tap sum."""
     from oracle import oracle as O
     from mnc_b200 import ops, dense
-    rng = np.random.default_rng(8)
-    C, H, W = 64, 38, 63
-    feat = np.maximum(rng.normal(size=(2, C, H, W)), 0).astype(np.float32)
+    rng = np.random.default_rng(8 if C == 64 else C + P)
+    H, W = 38, 63
+    feat = rng.normal(size=(2, C, H, W))
+    feat = (np.maximum(feat, 0) if C == 64 else feat).astype(np.float32)
     rois = _rois(50, 9, 1000, 600, levels=2)
     d_nhwc = torch.from_numpy(feat.transpose(0, 2, 3, 1).copy()).cuda()
     d_rois = torch.from_numpy(rois).cuda()
-    for fn, oracle_fn in ((ops.roi_pool_split, O.roi_pool), (ops.roi_sample_split, O.roi_warp)):
-        out = torch.zeros((2, 50, P, P, C), dtype=torch.bfloat16, device="cuda")
-        fn(d_nhwc, C, H, W, d_rois, P, out)
-        got = dense.merge(out).permute(0, 3, 1, 2).cpu().numpy()
-        want = oracle_fn(feat, rois, P, P)
-        assert util.rel_err(got, want) < 1e-4
-        assert np.all(got[2] == 0)   # the RoI outside the map
+    out = torch.zeros((2, 50, P, P, C), dtype=torch.bfloat16, device="cuda")
+    ops.roi_pool_split(d_nhwc, C, H, W, d_rois, P, out)
+    want = O.roi_pool(feat, rois, P, P)
+    want_split = dense.split(torch.from_numpy(want.transpose(0, 2, 3, 1).copy()))
+    assert torch.equal(out.cpu().view(torch.int16), want_split.view(torch.int16))
+    assert np.all(want[2] == 0)      # the RoI outside the map
+    out.zero_()
+    ops.roi_sample_split(d_nhwc, C, H, W, d_rois, P, out)
+    got = dense.merge(out).permute(0, 3, 1, 2).cpu().numpy().astype(np.float64)
+    want = O.roi_warp(feat, rois, P, P).astype(np.float64)
+    bound = 2.0 ** -16 * np.abs(want) + 2.0 ** -20 * O.roi_warp(np.abs(feat), rois, P, P)
+    assert np.all(np.abs(got - want) <= bound)
+    assert np.abs(want).max() > 0 and np.all(got[2] == 0)
 
 
 def test_faster_rcnn_engine_stagewise():

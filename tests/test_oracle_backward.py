@@ -134,15 +134,17 @@ def test_roi_pool_adjoint():
 
 
 # ---------------------------------------------------------------------------------- ROIWarping
-def _warp_geometry(roi, P, H, W):
+def _warp_geometry(roi, P, H, W, PW=None):
     """Per axis: the forward's clamped sample coordinate (float32) or None (outside the map), from
-    roi_warping_layer.cu:78-99 and :18-47, plus the backward's float32 window pieces (:197-233)."""
+    roi_warping_layer.cu:78-99 and :18-47, plus the backward's float32 window pieces (:197-233).
+    Pooled size P x P, or P x PW."""
+    PW = PW or P
     sw, sh, ew, eh = _roundf(roi[1:5] * f32(SS))
-    bin_f = (np.maximum(eh - sh, f32(0)) / f32(P), np.maximum(ew - sw, f32(0)) / f32(P))
-    bin_b = (np.maximum(eh - sh + f32(1), f32(1)) / f32(P), np.maximum(ew - sw + f32(1), f32(1)) / f32(P))
+    bin_f = (np.maximum(eh - sh, f32(0)) / f32(P), np.maximum(ew - sw, f32(0)) / f32(PW))
+    bin_b = (np.maximum(eh - sh + f32(1), f32(1)) / f32(P), np.maximum(ew - sw + f32(1), f32(1)) / f32(PW))
     samples = []
-    for start, b, dim in ((sh, bin_f[0], H), (sw, bin_f[1], W)):
-        xs = start + np.arange(P, dtype=np.float32) * b
+    for start, b, dim, n in ((sh, bin_f[0], H, P), (sw, bin_f[1], W, PW)):
+        xs = start + np.arange(n, dtype=np.float32) * b
         ok = ~((xs < -0.5) | (xs > dim - 0.5))
         a = np.maximum(xs, f32(0))
         a = np.where(a.astype(np.int64) >= dim - 1, f32(dim - 1), a)

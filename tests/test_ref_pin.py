@@ -176,21 +176,31 @@ def _warp_inputs(R, seed, B=2, C=24, H=38, W=63):
     return feat, np.vstack([edge, rois]).astype(np.float32)
 
 
-@pytest.mark.parametrize("P", [28, 14, 7])
-def test_roi_warping_three_way(P):
+# (ph, pw, C): the three fast paths at 24 channels, the generic kernel at a non-square and at the
+# largest size, and a channel count that is no multiple of the row walk's 32-channel CTAs
+WARP_PIN_SIZES = [pytest.param(P, P, 24, id=str(P)) for P in (28, 14, 7)] + [
+    pytest.param(9, 5, 24, id="9x5"), pytest.param(32, 32, 24, id="32x32"), pytest.param(28, 28, 72, id="C72-28")]
+
+
+def _pin_seed(P, PW, C):
+    return P if (PW, C) == (P, 24) else 1000 * C + 10 * P + PW
+
+
+@pytest.mark.parametrize("P,PW,C", WARP_PIN_SIZES)
+def test_roi_warping_three_way(P, PW, C):
     """ROIWarpingLayer::Forward_gpu (roi_warping_layer.cu:67-122) == oracle == mnc_roi_warp_nchw."""
     import torch
     from oracle import oracle as O
     from mnc_b200 import ops
     L = _layers()
-    feat, rois = _warp_inputs(120, seed=P)
+    feat, rois = _warp_inputs(120, seed=_pin_seed(P, PW, C), C=C)
     B, C, H, W = feat.shape
     R = rois.shape[0]
-    ref_out = np.zeros((R, C, P, P), np.float32)
-    assert L.ref_roi_warp(_p(feat), B, C, H, W, _p(rois), R, P, P, ctypes.c_float(0.0625), _p(ref_out)) == 0
+    ref_out = np.zeros((R, C, P, PW), np.float32)
+    assert L.ref_roi_warp(_p(feat), B, C, H, W, _p(rois), R, P, PW, ctypes.c_float(0.0625), _p(ref_out)) == 0
     assert np.abs(ref_out).max() > 0
-    orc = O.roi_warp(feat, rois, P, P)
-    got = ops.roi_warp_nchw(torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda(), P, P).cpu().numpy()
+    orc = O.roi_warp(feat, rois, P, PW)
+    got = ops.roi_warp_nchw(torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda(), P, PW).cpu().numpy()
     # nvcc fuses `start + p * bin` and the 4-tap sum of the reference source into FMAs; a 1-ulp
     # sample coordinate moves a value by ~1e-5 of the map's range.  The oracle and our kernel keep
     # every operation separately rounded, and equal the reference compiled with -fmad=false bit
@@ -199,7 +209,7 @@ def test_roi_warping_three_way(P):
     assert util.rel_err(got, ref_out) < 2e-5, "CUDA path differs from reference ROIWarping"
     assert np.array_equal(ref_out == 0, orc == 0)      # out-of-map samples in the same places
     nofma = np.zeros_like(ref_out)
-    assert _layers(True).ref_roi_warp(_p(feat), B, C, H, W, _p(rois), R, P, P, ctypes.c_float(0.0625),
+    assert _layers(True).ref_roi_warp(_p(feat), B, C, H, W, _p(rois), R, P, PW, ctypes.c_float(0.0625),
                                       _p(nofma)) == 0
     assert np.array_equal(orc, nofma), "oracle != reference ROIWarping built with -fmad=false"
     assert np.array_equal(got, nofma), "CUDA path != reference ROIWarping built with -fmad=false"

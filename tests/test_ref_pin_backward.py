@@ -17,7 +17,7 @@ import numpy as np
 import pytest
 
 from tests import util
-from tests.test_ref_pin import _p, _warp_inputs
+from tests.test_ref_pin import WARP_PIN_SIZES, _p, _pin_seed, _warp_inputs
 from tests.test_oracle_backward import _roundf, _warp_geometry
 
 pytestmark = pytest.mark.gpu
@@ -33,51 +33,51 @@ def _layers(nofma=False):
     return ctypes.CDLL(so)
 
 
-def _coord_safe(rois, P, H, W):
+def _coord_safe(rois, P, H, W, PW=None):
     """RoIs the reference's coordinate kernel handles inside its buffers."""
     ok = np.zeros(len(rois), bool)
     for i, roi in enumerate(rois):
         sw, sh, ew, eh = (int(v) for v in _roundf(roi[1:5] * np.float32(SS)))
-        _, _, ((_, okh), (_, okw)) = _warp_geometry(roi, P, H, W)
+        _, _, ((_, okh), (_, okw)) = _warp_geometry(roi, P, H, W, PW)
         ok[i] = okh.all() and okw.all() and sh <= eh and sw <= ew
     return ok
 
 
-def _ref_warp(L, feat, rois, top, P, pd1):
+def _ref_warp(L, feat, rois, top, P, pd1, PW=None):
     B, C, H, W = feat.shape
     R = rois.shape[0]
     fd = np.zeros_like(feat)
     rd = np.zeros((R, 5), np.float32)
-    assert L.ref_roi_warp_backward(_p(feat), B, C, H, W, _p(rois), R, P, P, ctypes.c_float(SS),
+    assert L.ref_roi_warp_backward(_p(feat), B, C, H, W, _p(rois), R, P, PW or P, ctypes.c_float(SS),
                                    _p(top), 1, int(pd1), _p(fd), _p(rd), 0, None) == 0
     return fd, rd
 
 
-@pytest.mark.parametrize("P", [28, 14, 7])
-def test_roi_warping_backward_three_way(P):
+@pytest.mark.parametrize("P,PW,C", WARP_PIN_SIZES)
+def test_roi_warping_backward_three_way(P, PW, C):
     import torch
     from oracle import oracle_backward as OB
     from mnc_b200 import ops
-    feat, rois = _warp_inputs(60, seed=P)
+    feat, rois = _warp_inputs(60, seed=_pin_seed(P, PW, C), C=C)
     B, C, H, W = feat.shape
-    rng = np.random.default_rng(P)
-    top = rng.standard_normal((rois.shape[0], C, P, P)).astype(np.float32)
-    want_f, want_r, mag = OB.roi_warp_backward(feat, rois, top, P, P, want_abs=True)
+    rng = np.random.default_rng(_pin_seed(P, PW, C))
+    top = rng.standard_normal((rois.shape[0], C, P, PW)).astype(np.float32)
+    want_f, want_r, mag = OB.roi_warp_backward(feat, rois, top, P, PW, want_abs=True)
     fd, rd = ops.roi_warp_backward_nchw(torch.from_numpy(feat).cuda(), torch.from_numpy(rois).cuda(),
-                                        torch.from_numpy(top).cuda(), P, P)
+                                        torch.from_numpy(top).cuda(), P, PW)
     fd, rd = fd.cpu().numpy(), rd.cpu().numpy()
     # feature gradient, every RoI (edge RoIs included), propagate_down = (1, 0)
-    nf_f, _ = _ref_warp(_layers(True), feat, rois, top, P, False)
+    nf_f, _ = _ref_warp(_layers(True), feat, rois, top, P, False, PW)
     assert np.array_equal(nf_f, want_f), "oracle != reference ROIWarping backward (-fmad=false)"
     assert np.array_equal(nf_f, fd), "CUDA != reference ROIWarping backward (-fmad=false)"
-    df_f, _ = _ref_warp(_layers(), feat, rois, top, P, False)
+    df_f, _ = _ref_warp(_layers(), feat, rois, top, P, False, PW)
     assert util.rel_err(fd, df_f) < 1e-4
     # coordinate gradient on the RoIs the reference's kernel handles inside its buffers
-    safe = _coord_safe(rois, P, H, W)
+    safe = _coord_safe(rois, P, H, W, PW)
     assert safe.sum() >= 30
     sr, st = np.ascontiguousarray(rois[safe]), np.ascontiguousarray(top[safe])
     for L in (_layers(True), _layers()):
-        f2, r2 = _ref_warp(L, feat, sr, st, P, True)
+        f2, r2 = _ref_warp(L, feat, sr, st, P, True, PW)
         assert np.all(r2[:, 0] == 0)
         assert np.all(np.abs(r2 - want_r[safe]) <= 1e-5 * mag[safe] + 1e-30)
         assert np.all(np.abs(r2 - rd[safe]) <= 1e-5 * mag[safe] + 1e-30)
