@@ -3,8 +3,10 @@
 // cv2.resize(fx = fy = scale, INTER_LINEAR), HWC -> NCHW blob.
 //
 // OpenCV's float INTER_LINEAR rule is restated (OpenCV is a dependency of the reference, not part
-// of it): source coordinate fx = (dx + 0.5) / scale - 0.5 in double, sx = floor(fx); sx < 0 -> (0, frac 0);
-// sx >= W-1 -> (W-1, frac 0); horizontal interpolation first, then vertical, in fp32.
+// of it): source coordinate fx = fma(dx + 0.5, 1 / scale, -0.5) in double, sx = floor(fx); sx < 0 ->
+// (0, frac 0); sx >= W-1 -> (W-1, frac 0); horizontal interpolation first, then vertical, in fp32
+// with separately rounded products and sums.  This is the device's rule, pinned bit for bit by
+// tests/cv_resize.py; cv2's own bits depend on whether IPP runs and on the CPU (DESIGN.md §6).
 #include <cuda_runtime.h>
 #include <cstdint>
 
@@ -18,9 +20,10 @@ struct LinTap {
 };
 
 __device__ __forceinline__ LinTap lin_tap(int d, double inv_scale, int n) {
-  // the fraction is taken in double and rounded once (OpenCV 4.x resize.cpp; an fp32 coordinate
-  // would lose 1e-5 of the fraction at x ~ 200 and 3e-3 of a pixel value -- measured against cv2)
-  const double fd = (d + 0.5) * inv_scale - 0.5;
+  // the coordinate is one fused multiply-add in double (written out, so that the rule does not
+  // depend on nvcc's contraction) and the fraction is rounded to fp32 once; an fp32 coordinate
+  // would lose 1e-5 of the fraction at x ~ 200 and 3e-3 of a pixel value -- measured against cv2
+  const double fd = fma(d + 0.5, inv_scale, -0.5);
   int s = static_cast<int>(floor(fd));
   float f = static_cast<float>(fd - s);
   if (s < 0) {

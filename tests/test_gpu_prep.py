@@ -1,10 +1,14 @@
-"""Device-side prep_im_for_blob + im_list_to_blob (lib/utils/blob.py:17-50) vs cv2 (the reference's
-own resize): golden fixtures made with cv2 (tests/golden/make_golden.py) and a live cv2 call."""
+"""Device-side prep_im_for_blob + im_list_to_blob (lib/utils/blob.py:17-50): bit for bit against the
+float32 model of the device's resize rule (tests/cv_resize.py), and within 1e-4 of cv2 (the
+reference's own resize, whose bits depend on IPP and the CPU): golden fixtures made with cv2
+(tests/golden/make_golden.py) and a live cv2 call."""
 import os
 
 import numpy as np
 import pytest
 import torch
+
+from tests import cv_resize as C
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -25,6 +29,8 @@ def test_prep_matches_cv2_golden(name):
     assert ops.im_scale_for(im.shape, int(tgt), int(mx)) == sc
     got = _run(im, float(sc))
     assert got.shape == want.shape
+    model = C.prep(im[None], float(sc), ops.PIXEL_MEANS)[0].transpose(1, 2, 0)
+    assert np.array_equal(got, model)
     # fp32 bilinear on values of magnitude <= 255: agreement to a few ulp of 255
     assert np.abs(got - want).max() < 1e-4
 
@@ -37,6 +43,8 @@ def test_prep_voc_sized_image_and_identity_scale():
     assert sc == 1.6
     got = _run(im, sc)
     assert got.shape == (600, 800, 3) and np.abs(got - want).max() < 1e-4
+    from mnc_b200 import ops
+    assert np.array_equal(got, C.prep(im[None], sc, ops.PIXEL_MEANS)[0].transpose(1, 2, 0))
     im2 = O.synthetic_image(0, 600, 1000)
     blob, info = O.prep_blob(im2)             # scale 1.0: pure mean subtraction + transpose
     got2 = _run(im2, 1.0)

@@ -85,7 +85,9 @@ def test_matches_reference_fixtures(name):
 
 
 def test_random_cases_match_oracle():
-    near = 0
+    """Mask targets and MaskLayer labels equal the model of the device's resize rule exactly; the
+    oracle (OpenCV's resize) may differ only at samples within CV2_ULPS of 0.4f."""
+    from tests import cv_resize as C
     for seed in range(24):
         kw = dict(H=600, W=1000, im_scale=1.6, n=64, G=3 + seed % 18) if seed % 2 else \
             dict(H=480, W=640, im_scale=1.0 + 0.05 * seed, n=32 + seed, G=2 + seed % 5)
@@ -98,20 +100,17 @@ def test_random_cases_match_oracle():
         wrd, wbd = T.stage_bridge_backward(td, want, case["rois"], case["bbox_pred"], clip)
         f = dict(case, top_diff=td)
         out, rd, bd = _device(f, pre, clip)
-        tv = T.target_values(case, want)
-        near += int(np.sum(np.abs(tv - 0.4) < 1e-6))
-        got = out["mask_targets"].cpu().numpy()
-        diff = got != want["mask_targets"]
-        assert diff.sum() <= near, (seed, diff.sum(), near)
-        want["mask_targets"] = got if diff.sum() else want["mask_targets"]
+        gm = case["gt_masks"].astype(np.float32)
+        model, _ = C.mask_targets(want["gt_mask_info"], want["nfg"], gm)
+        close = C.mask_targets_cv2_band(want["gt_mask_info"], want["nfg"], gm)
+        assert np.all(close[model != want["mask_targets"]]), seed
+        want["mask_targets"] = model
         _compare(out, rd, bd, want, wrd, wbd, case)
         pred = T.mask_predictions(seed, want["mask_targets"], want["gt_mask_info"])
         labels = _mask_layer(pred, case["gt_masks"], want["gt_mask_info"]).cpu().numpy()
-        rv = T.resize_values(pred, want["gt_mask_info"])
+        assert np.array_equal(labels, C.mask_layer(pred, gm, want["gt_mask_info"])), seed
         wl = T.mask_layer_forward(pred, case["gt_masks"], want["gt_mask_info"]).reshape(-1)
-        if np.abs(rv - 0.4).min(initial=1) >= 1e-6:
-            assert np.array_equal(labels, wl), seed
-    print("random-case mask samples within 1e-6 of BINARIZE_THRESH: %d" % near)
+        assert np.all(C.mask_layer_cv2_band(pred, want["gt_mask_info"])[labels != wl]), seed
 
 
 def _case_tensors(seed=3):
