@@ -26,11 +26,12 @@ extern "C" {
 
 #define MNC_OK 0
 #define MNC_ERR_ARG 1    /* invalid argument / unsupported shape */
-#define MNC_ERR_CUDA 2   /* a CUDA runtime call or launch failed (see mnc_last_cuda_error) */
+#define MNC_ERR_CUDA 2   /* a CUDA runtime call or launch failed; mnc_last_cuda_error names its error */
 #define MNC_ERR_DRIVER 3 /* cuTensorMapEncodeTiled unavailable or failed */
 #define MNC_ERR_NOGPU 4  /* no CUDA device visible */
 
-/* Library identity / diagnostics. */
+/* Library identity / diagnostics.  mnc_last_cuda_error: the error behind the calling thread's last
+ * MNC_ERR_CUDA; a success keeps it, the next failure replaces it, "no error" before any failure. */
 int mnc_abi_version(void);
 const char* mnc_last_cuda_error(void);
 int mnc_device_count(void);

@@ -2,11 +2,12 @@
 #include <cuda_runtime.h>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 
 extern "C" int mnc_abi_version(void) { return 1; }
 
 extern "C" const char* mnc_last_cuda_error(void) {
-  return cudaGetErrorString(cudaGetLastError());
+  return cudaGetErrorString(mnc::last_cuda_error);
 }
 
 extern "C" int mnc_device_count(void) {

@@ -6,6 +6,7 @@
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 
 namespace mnc {
 
@@ -387,14 +388,6 @@ __global__ void split_to_f32_kernel(const __nv_bfloat16* __restrict__ in_hi,
     out[i] = bf2f(in_hi[i]) + bf2f(in_lo[i]);
 }
 
-static inline int grid_for(long long n, int block, int cap = 132 * 16) {
-  long long g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-static inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
-
 }  // namespace mnc
 
 using namespace mnc;
@@ -474,13 +467,13 @@ extern "C" int mnc_nchw_to_split(const float* in_nchw, int batch, int C, int H, 
 
 extern "C" int mnc_f32_to_split(const float* in, long long n, void* out_hi, void* out_lo,
                                 void* stream) {
-  f32_to_split_kernel<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  f32_to_split_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       in, n, static_cast<__nv_bfloat16*>(out_hi), static_cast<__nv_bfloat16*>(out_lo));
   return check_launch();
 }
 extern "C" int mnc_split_to_f32(const void* in_hi, const void* in_lo, long long n, float* out,
                                 void* stream) {
-  split_to_f32_kernel<<<grid_for(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  split_to_f32_kernel<<<grid_for(n, 256, 132 * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(in_hi), static_cast<const __nv_bfloat16*>(in_lo), n, out);
   return check_launch();
 }

@@ -886,14 +886,15 @@ static int launch_igemm(const Maps& m, const IgemmArgs& a, int max_ctas, cudaStr
   using Cfg = IgemmCfg<BN, TH>;
   auto kern = igemm_tc_kernel<TH, TW, BN, PM>;
   static SmemGrant grant;
-  if (!ensure_dynamic_smem(kern, Cfg::kSmemBytes, grant)) return MNC_ERR_CUDA;
+  const int rc = ensure_dynamic_smem(kern, Cfg::kSmemBytes, grant);
+  if (rc != MNC_OK) return rc;
   const int total = a.split_k * a.tiles_n * a.batch * a.tiles_h * a.tiles_w;
   int grid = sm_count();
   if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
   if (total < grid) grid = total;
   kern<<<grid, 384, Cfg::kSmemBytes, stream>>>(m.a[0], m.a[1], m.a[2], m.b[0], m.b[1], m.b[2], m.o[0],
                                                m.o[1], m.o[2], a);
-  return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA;
+  return check_launch();
 }
 
 }  // namespace mnc
@@ -1081,13 +1082,13 @@ extern "C" int mnc_conv1_1_tc2(const float* data_nchw, int batch, int H, int W, 
   to_x = to_lo;
   if (out_mode == 4 && (rc = make_out_map(&to_x, out2, a.batch, 1, W, 64, 64, 1, 128, 1)) != MNC_OK) return rc;
   static SmemGrant grant;
-  if (!ensure_dynamic_smem(conv1_1_tc_kernel, kC11Smem, grant)) return MNC_ERR_CUDA;
+  if ((rc = ensure_dynamic_smem(conv1_1_tc_kernel, kC11Smem, grant)) != MNC_OK) return rc;
   const int total = a.batch * a.tiles_w;
   int grid = sm_count();
   if (total < grid) grid = total;
   conv1_1_tc_kernel<<<grid, kC11Threads, kC11Smem, stream>>>(data_nchw, batch, H, W, tb, to_hi, to_lo,
                                                              to_x, a);
-  return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA;
+  return check_launch();
 }
 
 extern "C" int mnc_conv1_1_tc(const float* data_nchw, int batch, int H, int W, const void* w_stacked,

@@ -18,14 +18,13 @@
 #include <cuda_runtime.h>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 
 namespace mnc {
 namespace {
 
 constexpr int kT = 1024;              // threads of the one-CTA kernels
 constexpr int kEwThreads = 256;       // element-wise backward
-
-inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 __device__ __forceinline__ int valid_rows(const int* n_valid, int num) {
   if (!n_valid) return num;

@@ -17,6 +17,7 @@
 // Per-pixel arithmetic mirrors the reference expression by expression (same last-row / last-col
 // nearest rule, same W/2, H/2 defaults for an empty mask).
 #include <cuda_runtime.h>
+#include <atomic>
 #include <climits>
 #include <cstdint>
 
@@ -630,8 +631,6 @@ vote_candidates_kernel(const float* __restrict__ boxes, const float* __restrict_
   }
 }
 
-static inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
-
 }  // namespace mnc
 
 using namespace mnc;
@@ -660,9 +659,10 @@ extern "C" int mnc_mv_device(const float* boxes, const float* masks, int nb, int
   const int smem = nb * (16 + 4 + 4 + 8 + 4);
   if (smem > 200 * 1024) return MNC_ERR_ARG;
   static SmemGrant grant_agg, grant_fin;   // (static shared memory counts against the 48 KB default)
-  if (!ensure_dynamic_smem(mv_aggregate_kernel, smem, grant_agg) ||
-      !ensure_dynamic_smem(mv_finalize_kernel, smem, grant_fin))
-    return MNC_ERR_CUDA;
+  int rc;
+  if ((rc = ensure_dynamic_smem(mv_aggregate_kernel, smem, grant_agg)) != MNC_OK ||
+      (rc = ensure_dynamic_smem(mv_finalize_kernel, smem, grant_fin)) != MNC_OK)
+    return rc;
   const int total = batch * max_results;
   int* unit = bbox_ws + static_cast<long long>(total) * 4;   // [batch] flags after the boxes
   mv_init_bbox_kernel<<<(total + 255) / 256, 256, 0, stream>>>(bbox_ws, total, unit, batch);
@@ -691,13 +691,15 @@ extern "C" int mnc_vote_select(const float* scores, int nb, int ncls, const int*
                                int* overflow, void* stream_) {
   const int cap = (ncls - 1) * max_per_image;
   const int smem = cap * 12 + (ncls + 1) * 4;
-  // without an opt-in, the kernel's static shared memory and the dynamic part share 48 KB
-  static const int static_smem = [] {
+  // without an opt-in, the kernel's static shared memory and the dynamic part share 48 KB; only a
+  // successful query is kept, a failed one is tried again on the next call
+  static std::atomic<int> static_smem{-1};
+  if (static_smem < 0) {
     cudaFuncAttributes a{};
-    return cudaFuncGetAttributes(&a, vote_select_kernel) == cudaSuccess
-               ? static_cast<int>(a.sharedSizeBytes) : -1;
-  }();
-  if (static_smem < 0) return MNC_ERR_CUDA;
+    const int rc = cuda_status(cudaFuncGetAttributes(&a, vote_select_kernel));
+    if (rc != MNC_OK) return rc;
+    static_smem = static_cast<int>(a.sharedSizeBytes);
+  }
   if (smem + static_smem > 48 * 1024) return MNC_ERR_ARG;
   vote_select_kernel<<<batch, 1024, smem, static_cast<cudaStream_t>(stream_)>>>(
       scores, nb, ncls, order, keep, keep_stride, num_keep, max_per_image, max_results,
@@ -738,9 +740,9 @@ extern "C" int mnc_mv_host(const float* all_boxes, const float* all_masks, int a
     return MNC_ERR_ARG;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return MNC_ERR_NOGPU;
-  int cur = 0;
+  int cur = 0, rc;
   cudaGetDevice(&cur);
-  if (cur != device_id && cudaSetDevice(device_id) != cudaSuccess) return MNC_ERR_CUDA;
+  if (cur != device_id && (rc = cuda_status(cudaSetDevice(device_id))) != MNC_OK) return rc;
   const size_t nb = all_boxes_num, mm = static_cast<size_t>(mask_size) * mask_size;
   auto al = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
   const size_t o_boxes = 0;
@@ -756,24 +758,26 @@ extern "C" int mnc_mv_host(const float* all_boxes, const float* all_masks, int a
   const size_t o_obox = o_omask + al(static_cast<size_t>(result_num) * mm * 4);
   const size_t total = o_obox + al(static_cast<size_t>(result_num) * 16);
   char* base = nullptr;
-  if (cudaMalloc(&base, total) != cudaSuccess) return MNC_ERR_CUDA;
-  int rc = MNC_OK;
+  rc = cuda_status(cudaMalloc(&base, total));
+  if (rc != MNC_OK) return rc;
   int* h_begin = new int[result_num];
   for (int n = 0; n < result_num; ++n) h_begin[n] = (n == 0) ? 0 : candidate_start[n - 1];
   const int h_hw[2] = {image_height, image_width};
-  bool ok = true;
-  ok &= cudaMemcpy(base + o_boxes, all_boxes, nb * box_dim * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-  ok &= cudaMemcpy(base + o_masks, all_masks, nb * mm * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+  auto copy = [&rc](void* dst, const void* src, size_t bytes, cudaMemcpyKind kind) {
+    if (rc == MNC_OK) rc = cuda_status(cudaMemcpy(dst, src, bytes, kind));
+  };
+  copy(base + o_boxes, all_boxes, nb * box_dim * 4, cudaMemcpyHostToDevice);
+  copy(base + o_masks, all_masks, nb * mm * 4, cudaMemcpyHostToDevice);
   if (candidate_num > 0) {
-    ok &= cudaMemcpy(base + o_inds, candidate_inds, static_cast<size_t>(candidate_num) * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-    ok &= cudaMemcpy(base + o_wgt, candidate_weights, static_cast<size_t>(candidate_num) * 4, cudaMemcpyHostToDevice) == cudaSuccess;
+    copy(base + o_inds, candidate_inds, static_cast<size_t>(candidate_num) * 4, cudaMemcpyHostToDevice);
+    copy(base + o_wgt, candidate_weights, static_cast<size_t>(candidate_num) * 4, cudaMemcpyHostToDevice);
   }
-  ok &= cudaMemcpy(base + o_begin, h_begin, static_cast<size_t>(result_num) * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-  ok &= cudaMemcpy(base + o_end, candidate_start, static_cast<size_t>(result_num) * 4, cudaMemcpyHostToDevice) == cudaSuccess;
-  ok &= cudaMemcpy(base + o_nres, &result_num, 4, cudaMemcpyHostToDevice) == cudaSuccess;
-  ok &= cudaMemcpy(base + o_hw, h_hw, 8, cudaMemcpyHostToDevice) == cudaSuccess;
+  copy(base + o_begin, h_begin, static_cast<size_t>(result_num) * 4, cudaMemcpyHostToDevice);
+  copy(base + o_end, candidate_start, static_cast<size_t>(result_num) * 4, cudaMemcpyHostToDevice);
+  copy(base + o_nres, &result_num, 4, cudaMemcpyHostToDevice);
+  copy(base + o_hw, h_hw, 8, cudaMemcpyHostToDevice);
   delete[] h_begin;
-  if (ok) {
+  if (rc == MNC_OK)
     rc = mnc_mv_device(reinterpret_cast<float*>(base + o_boxes),
                        reinterpret_cast<float*>(base + o_masks), all_boxes_num, box_dim, mask_size,
                        reinterpret_cast<int*>(base + o_inds),
@@ -783,13 +787,9 @@ extern "C" int mnc_mv_host(const float* all_boxes, const float* all_masks, int a
                        reinterpret_cast<int*>(base + o_hw), reinterpret_cast<int*>(base + o_bbox),
                        reinterpret_cast<float*>(base + o_omask),
                        reinterpret_cast<int*>(base + o_obox), nullptr);
-    if (rc == MNC_OK) {
-      ok &= cudaMemcpy(finalize_output_mask, base + o_omask, static_cast<size_t>(result_num) * mm * 4, cudaMemcpyDeviceToHost) == cudaSuccess;
-      ok &= cudaMemcpy(finalize_output_box, base + o_obox, static_cast<size_t>(result_num) * 16, cudaMemcpyDeviceToHost) == cudaSuccess;
-    }
-  }
+  copy(finalize_output_mask, base + o_omask, static_cast<size_t>(result_num) * mm * 4, cudaMemcpyDeviceToHost);
+  copy(finalize_output_box, base + o_obox, static_cast<size_t>(result_num) * 16, cudaMemcpyDeviceToHost);
   cudaFree(base);
-  if (!ok) return MNC_ERR_CUDA;
   return rc;
 }
 
@@ -824,19 +824,19 @@ extern "C" int mnc_bbox_overlaps_host(const double* boxes, int N, const double* 
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return MNC_ERR_NOGPU;
   double *d_b = nullptr, *d_q = nullptr, *d_o = nullptr;
-  bool ok = cudaMalloc(&d_b, sizeof(double) * 4 * N) == cudaSuccess &&
-            cudaMalloc(&d_q, sizeof(double) * 4 * K) == cudaSuccess &&
-            cudaMalloc(&d_o, sizeof(double) * static_cast<size_t>(N) * K) == cudaSuccess;
-  if (ok) {
-    ok &= cudaMemcpy(d_b, boxes, sizeof(double) * 4 * N, cudaMemcpyHostToDevice) == cudaSuccess;
-    ok &= cudaMemcpy(d_q, query, sizeof(double) * 4 * K, cudaMemcpyHostToDevice) == cudaSuccess;
-    const long long total = static_cast<long long>(N) * K;
+  const long long total = static_cast<long long>(N) * K;
+  int rc = cuda_status(cudaMalloc(&d_b, sizeof(double) * 4 * N));
+  if (rc == MNC_OK) rc = cuda_status(cudaMalloc(&d_q, sizeof(double) * 4 * K));
+  if (rc == MNC_OK) rc = cuda_status(cudaMalloc(&d_o, sizeof(double) * total));
+  if (rc == MNC_OK) rc = cuda_status(cudaMemcpy(d_b, boxes, sizeof(double) * 4 * N, cudaMemcpyHostToDevice));
+  if (rc == MNC_OK) rc = cuda_status(cudaMemcpy(d_q, query, sizeof(double) * 4 * K, cudaMemcpyHostToDevice));
+  if (rc == MNC_OK) {
     mnc::bbox_overlaps_kernel<<<static_cast<unsigned>((total + 255) / 256), 256>>>(d_b, N, d_q, K, d_o);
-    ok &= cudaGetLastError() == cudaSuccess;
-    ok &= cudaMemcpy(out, d_o, sizeof(double) * static_cast<size_t>(N) * K, cudaMemcpyDeviceToHost) == cudaSuccess;
+    rc = check_launch();
   }
+  if (rc == MNC_OK) rc = cuda_status(cudaMemcpy(out, d_o, sizeof(double) * total, cudaMemcpyDeviceToHost));
   cudaFree(d_b);
   cudaFree(d_q);
   cudaFree(d_o);
-  return ok ? MNC_OK : MNC_ERR_CUDA;
+  return rc;
 }

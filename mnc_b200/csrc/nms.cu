@@ -797,8 +797,6 @@ __global__ void gather_boxes_kernel(const float* __restrict__ src, int src_strid
   *reinterpret_cast<float4*>(dst + (static_cast<long long>(prob) * n_out + k) * 4) = v;
 }
 
-static inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
-
 }  // namespace mnc
 
 using namespace mnc;
@@ -874,7 +872,8 @@ extern "C" int mnc_rank_sort_desc(const float* keys, long long outer_stride,
     while (np2 < n) np2 <<= 1;
     const int smem = np2 * 6;
     static SmemGrant grant;   // always opt in: static shared memory counts against the 48 KB default
-    if (!ensure_dynamic_smem(bitonic_sort_desc_kernel, smem, grant)) return MNC_ERR_CUDA;
+    const int rc = ensure_dynamic_smem(bitonic_sort_desc_kernel, smem, grant);
+    if (rc != MNC_OK) return rc;
     bitonic_sort_desc_kernel<<<problems, 1024, smem, static_cast<cudaStream_t>(stream_)>>>(
         keys, outer_stride, inner_stride, inner, key_stride, valid, n, np2, order, n_valid);
     return check_launch();
@@ -896,7 +895,8 @@ extern "C" int mnc_topk_sort_desc(const float* keys, long long outer_stride, lon
   const size_t smem = static_cast<size_t>(np2) * 8 + static_cast<size_t>(n) * 4;
   if (smem > 200 * 1024) return MNC_ERR_ARG;   // callers fall back to mnc_rank_sort_desc
   static SmemGrant grant;
-  if (!ensure_dynamic_smem(topk_sort_desc_kernel, static_cast<int>(smem), grant)) return MNC_ERR_CUDA;
+  const int rc = ensure_dynamic_smem(topk_sort_desc_kernel, static_cast<int>(smem), grant);
+  if (rc != MNC_OK) return rc;
   topk_sort_desc_kernel<<<problems, kTopkThreads, smem, static_cast<cudaStream_t>(stream_)>>>(
       keys, outer_stride, inner_stride, inner, key_stride, valid, n, k, np2, order, order_stride,
       n_out);
@@ -935,7 +935,8 @@ int ensure_scratch(size_t bytes, int device) {
     if (g_scratch.dev) cudaFree(g_scratch.dev);
     g_scratch.dev = nullptr;
     g_scratch.bytes = 0;
-    if (cudaMalloc(&g_scratch.dev, bytes) != cudaSuccess) return MNC_ERR_CUDA;
+    const int rc = cuda_status(cudaMalloc(&g_scratch.dev, bytes));
+    if (rc != MNC_OK) return rc;
     g_scratch.bytes = bytes;
     g_scratch.device = device;
   }
@@ -952,31 +953,31 @@ extern "C" int mnc_nms_host(int* keep_out, int* num_out, const float* boxes_host
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return MNC_ERR_NOGPU;
-  int cur = 0;
+  int cur = 0, rc;
   cudaGetDevice(&cur);
-  if (cur != device_id && cudaSetDevice(device_id) != cudaSuccess) return MNC_ERR_CUDA;
+  if (cur != device_id && (rc = cuda_status(cudaSetDevice(device_id))) != MNC_OK) return rc;
   const size_t box_bytes = static_cast<size_t>(boxes_num) * boxes_dim * sizeof(float);
   const size_t box_al = (box_bytes + 255) & ~static_cast<size_t>(255);
   const size_t mask_bytes = static_cast<size_t>(mnc_nms_workspace_bytes(boxes_num, 1));
   const size_t keep_bytes = (static_cast<size_t>(boxes_num) + 1) * sizeof(int);
-  int rc = ensure_scratch(box_al + mask_bytes + keep_bytes + 256, device_id);
+  rc = ensure_scratch(box_al + mask_bytes + keep_bytes + 256, device_id);
   if (rc != MNC_OK) return rc;
   char* base = static_cast<char*>(g_scratch.dev);
   float* d_boxes = reinterpret_cast<float*>(base);
   void* d_mask = base + box_al;
   int* d_keep = reinterpret_cast<int*>(base + box_al + mask_bytes);
   int* d_num = d_keep + boxes_num;
-  if (cudaMemcpy(d_boxes, boxes_host, box_bytes, cudaMemcpyHostToDevice) != cudaSuccess)
-    return MNC_ERR_CUDA;
+  if ((rc = cuda_status(cudaMemcpy(d_boxes, boxes_host, box_bytes, cudaMemcpyHostToDevice))) != MNC_OK)
+    return rc;
   rc = mnc_nms_sorted(d_boxes, boxes_dim, 0, nullptr, boxes_num, 1, nms_overlap_thresh, boxes_num,
                       d_mask, d_keep, boxes_num, d_num, nullptr);
   if (rc != MNC_OK) return rc;
   int num = 0;
-  if (cudaMemcpy(&num, d_num, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
-    return MNC_ERR_CUDA;
+  if ((rc = cuda_status(cudaMemcpy(&num, d_num, sizeof(int), cudaMemcpyDeviceToHost))) != MNC_OK)
+    return rc;
   if (num > 0 &&
-      cudaMemcpy(keep_out, d_keep, sizeof(int) * num, cudaMemcpyDeviceToHost) != cudaSuccess)
-    return MNC_ERR_CUDA;
+      (rc = cuda_status(cudaMemcpy(keep_out, d_keep, sizeof(int) * num, cudaMemcpyDeviceToHost))) != MNC_OK)
+    return rc;
   *num_out = num;
   return MNC_OK;
 }
@@ -996,15 +997,15 @@ extern "C" int mnc_gpu_nms_host(int* keep_out, int* num_out, const float* dets_h
   }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return MNC_ERR_NOGPU;
-  int cur = 0;
+  int cur = 0, rc;
   cudaGetDevice(&cur);
-  if (cur != device_id && cudaSetDevice(device_id) != cudaSuccess) return MNC_ERR_CUDA;
+  if (cur != device_id && (rc = cuda_status(cudaSetDevice(device_id))) != MNC_OK) return rc;
   auto al = [](size_t b) { return (b + 255) & ~static_cast<size_t>(255); };
   const size_t dets_b = al(static_cast<size_t>(n) * dim * sizeof(float));
   const size_t sorted_b = al(static_cast<size_t>(n) * 4 * sizeof(float));
   const size_t ints_b = al((static_cast<size_t>(n) + 4) * sizeof(int));
   const size_t mask_b = al(static_cast<size_t>(mnc_nms_workspace_bytes(n, 1)));
-  int rc = ensure_scratch(dets_b + sorted_b + 2 * ints_b + mask_b + 256, device_id);
+  rc = ensure_scratch(dets_b + sorted_b + 2 * ints_b + mask_b + 256, device_id);
   if (rc != MNC_OK) return rc;
   char* base = static_cast<char*>(g_scratch.dev);
   float* d_dets = reinterpret_cast<float*>(base);
@@ -1012,9 +1013,9 @@ extern "C" int mnc_gpu_nms_host(int* keep_out, int* num_out, const float* dets_h
   int* d_order = reinterpret_cast<int*>(base + dets_b + sorted_b);       // [n] + n_valid + count
   int* d_keep = reinterpret_cast<int*>(base + dets_b + sorted_b + ints_b);  // [n] + num
   void* d_mask = base + dets_b + sorted_b + 2 * ints_b;
-  if (cudaMemcpy(d_dets, dets_host, static_cast<size_t>(n) * dim * sizeof(float),
-                 cudaMemcpyHostToDevice) != cudaSuccess)
-    return MNC_ERR_CUDA;
+  if ((rc = cuda_status(cudaMemcpy(d_dets, dets_host, static_cast<size_t>(n) * dim * sizeof(float),
+                                   cudaMemcpyHostToDevice))) != MNC_OK)
+    return rc;
   if ((rc = mnc_rank_sort_desc(d_dets + 4, 0, 0, 1, dim, nullptr, n, 1, d_order, d_order + n,
                                nullptr)) != MNC_OK)
     return rc;
@@ -1025,8 +1026,8 @@ extern "C" int mnc_gpu_nms_host(int* keep_out, int* num_out, const float* dets_h
                            d_keep + n, nullptr)) != MNC_OK)
     return rc;
   int num = 0;
-  if (cudaMemcpy(&num, d_keep + n, sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess)
-    return MNC_ERR_CUDA;
+  if ((rc = cuda_status(cudaMemcpy(&num, d_keep + n, sizeof(int), cudaMemcpyDeviceToHost))) != MNC_OK)
+    return rc;
   if (num > 0) {
     // keep (positions in the sorted list) -> original row indices, on the host: two small copies
     static thread_local int* h_order = nullptr;
@@ -1037,9 +1038,9 @@ extern "C" int mnc_gpu_nms_host(int* keep_out, int* num_out, const float* dets_h
       h_cap = h_order ? n : 0;
       if (!h_order) return MNC_ERR_ARG;
     }
-    if (cudaMemcpy(h_order, d_order, sizeof(int) * n, cudaMemcpyDeviceToHost) != cudaSuccess ||
-        cudaMemcpy(keep_out, d_keep, sizeof(int) * num, cudaMemcpyDeviceToHost) != cudaSuccess)
-      return MNC_ERR_CUDA;
+    if ((rc = cuda_status(cudaMemcpy(h_order, d_order, sizeof(int) * n, cudaMemcpyDeviceToHost))) != MNC_OK ||
+        (rc = cuda_status(cudaMemcpy(keep_out, d_keep, sizeof(int) * num, cudaMemcpyDeviceToHost))) != MNC_OK)
+      return rc;
     for (int i = 0; i < num; ++i) keep_out[i] = h_order[keep_out[i]];
   }
   *num_out = num;

@@ -11,6 +11,7 @@
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 
 namespace mnc {
 
@@ -79,5 +80,5 @@ extern "C" int mnc_prep_images(const unsigned char* img_bgr_hwc, int batch, int 
   mnc::prep_image_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       img_bgr_hwc, H, W, pixel_means3[0], pixel_means3[1], pixel_means3[2], 1.0 / scale, out_h,
       out_w, out_nchw);
-  return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA;
+  return mnc::check_launch();
 }

@@ -13,6 +13,7 @@
 
 #include "mnc_b200.h"
 #include "bbox_decode.cuh"
+#include "launch_util.h"
 
 namespace mnc {
 
@@ -282,8 +283,6 @@ __global__ void decode_class_boxes_kernel(const float* __restrict__ rois, int to
   *reinterpret_cast<float4*>(out + (static_cast<long long>(i) * ncls + c) * 4) =
       make_float4(o[0], o[1], o[2], o[3]);
 }
-
-static inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 }  // namespace mnc
 

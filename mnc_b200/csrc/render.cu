@@ -14,6 +14,7 @@
 
 #include "mnc_b200.h"
 #include "cv_resize.cuh"
+#include "launch_util.h"
 
 namespace mnc {
 
@@ -156,7 +157,7 @@ extern "C" int mnc_paste_instances(const float* boxes, int box_dim, const float*
   dim3 grid((W + 127) / 128, H, batch);
   mnc::paste_instances_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       boxes, box_dim, masks, cls, counts, max_n, mask_size, H, W, thresh, inst_img, cls_img, bgr);
-  return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA;
+  return mnc::check_launch();
 }
 
 extern "C" int mnc_binarize_masks(const int* rboxes, const float* masks, int n, int mask_size,
@@ -168,5 +169,5 @@ extern "C" int mnc_binarize_masks(const int* rboxes, const float* masks, int n, 
   if (gx > 1024) gx = 1024;
   mnc::binarize_masks_kernel<<<dim3(gx, n), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       rboxes, masks, mask_size, thresh, offsets, out);
-  return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA;
+  return mnc::check_launch();
 }

@@ -25,6 +25,7 @@
 #include <cuda_runtime.h>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 #include "roi_geom.cuh"
 
 namespace mnc {
@@ -36,8 +37,6 @@ constexpr int kSlab = 8;                         // channels per CTA, accumulate
 constexpr int kChunk = 16;                       // RoIs whose tables are staged at once
 constexpr int kCoordSlab = 64;                   // channels per CTA of the coordinate gradient
 constexpr int kCoordThreads = 256;
-
-inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 // Ordered compaction over the block (kTileThreads threads): returns how many threads have `hit`
 // set and gives each such thread its rank among them in `pos` (ranks follow thread order).  The
@@ -541,13 +540,6 @@ roi_pool_bwd_kernel(const float* __restrict__ rois, int R, int C, int H, int W, 
   }
 }
 
-inline int grid_for(long long n, int block, int cap) {
-  long long g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-
 inline dim3 tile_grid(int B, int C, int H, int W) {
   return dim3(((H + kTileH - 1) / kTileH) * ((W + kTileW - 1) / kTileW), (C + kSlab - 1) / kSlab, B);
 }
@@ -574,14 +566,15 @@ extern "C" int mnc_roi_warp_backward_nchw(const float* feat, int B, int C, int H
   if (rois_diff) {
     const int slabs = (C + kCoordSlab - 1) / kCoordSlab;
     double* partial = nullptr;
-    if (cudaMallocAsync(reinterpret_cast<void**>(&partial),
-                        sizeof(double) * 4 * static_cast<size_t>(R) * slabs, s) != cudaSuccess)
-      return MNC_ERR_CUDA;
+    int rc = cuda_status(cudaMallocAsync(reinterpret_cast<void**>(&partial),
+                                         sizeof(double) * 4 * static_cast<size_t>(R) * slabs, s));
+    if (rc != MNC_OK) return rc;
     roi_warp_bwd_coord_kernel<<<dim3(R, slabs), kCoordThreads, 0, s>>>(
         feat, B, C, H, W, rois, pooled_h, pooled_w, spatial_scale, top_diff, partial);
     roi_warp_bwd_coord_sum_kernel<<<grid_for(5LL * R, 256, 1 << 30), 256, 0, s>>>(partial, R, slabs, rois_diff);
-    const int rc = check_launch();
-    if (cudaFreeAsync(partial, s) != cudaSuccess || rc != MNC_OK) return MNC_ERR_CUDA;
+    rc = check_launch();
+    const int rc_free = cuda_status(cudaFreeAsync(partial, s));   // freed whether or not the launch failed
+    return rc != MNC_OK ? rc : rc_free;
   }
   return MNC_OK;
 }

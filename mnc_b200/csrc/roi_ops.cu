@@ -24,6 +24,7 @@
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 #include "roi_geom.cuh"
 #include "tri.cuh"
 
@@ -658,14 +659,6 @@ mask_pool_split_kernel(const __nv_bfloat16* __restrict__ f_hi, const __nv_bfloat
       st_split2(o_hi, o_lo, ((static_cast<long long>(r) * 7 + t) * 7 + jp) * C + c, best.x, best.y);
     }
   }
-}
-
-static inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
-static inline int grid_for(long long n, int block, int cap) {
-  long long g = (n + block - 1) / block;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
 }
 
 }  // namespace mnc

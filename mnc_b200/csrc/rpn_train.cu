@@ -19,6 +19,7 @@
 #include "mnc_b200.h"
 #include "bbox_decode.cuh"
 #include "mask_target.cuh"
+#include "launch_util.h"
 
 namespace mnc {
 namespace {
@@ -27,8 +28,6 @@ constexpr int kA = 9;                 // anchors per position (generate_anchors)
 constexpr int kSelThreads = 1024;
 constexpr int kMaskThreads = 256;
 constexpr int kMaxCats = 4;
-
-inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 struct AnchorTable {
   float v[kA][4];
@@ -654,8 +653,8 @@ extern "C" int mnc_proposal_backward(const float* top_diff, int R, const int* st
   if (R < 0 || H <= 0 || W <= 0 || clip_thresh < 0.f) return MNC_ERR_ARG;
   if (!bbox_pred_diff) return MNC_OK;
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (cudaMemsetAsync(bbox_pred_diff, 0, sizeof(float) * 4 * mnc::kA * H * W, s) != cudaSuccess)
-    return MNC_ERR_CUDA;
+  const int rc = mnc::cuda_status(cudaMemsetAsync(bbox_pred_diff, 0, sizeof(float) * 4 * mnc::kA * H * W, s));
+  if (rc != MNC_OK) return rc;
   if (R > 0)
     mnc::proposal_backward_kernel<<<(R + 127) / 128, 128, 0, s>>>(
         top_diff, R, state, rpn_bbox_pred, H, W, mnc::anchor_table(), clip_thresh, bbox_pred_diff);
@@ -762,7 +761,8 @@ extern "C" int mnc_anchor_target(
   const int T = H * W * mnc::kA;
   const mnc::AtWs ws = mnc::at_ws(workspace, T, G);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (cudaMemsetAsync(ws.gmax, 0, 8LL * G, s) != cudaSuccess) return MNC_ERR_CUDA;
+  const int rc = mnc::cuda_status(cudaMemsetAsync(ws.gmax, 0, 8LL * G, s));
+  if (rc != MNC_OK) return rc;
   const mnc::AnchorTable an = mnc::anchor_table();
   const int grid = (T + 255) / 256;
   mnc::anchor_overlaps_kernel<<<grid, 256, 0, s>>>(T, W, feat_stride, an, gt_boxes, G, im_info,

@@ -23,14 +23,13 @@
 #include "mnc_b200.h"
 #include "cv_resize.cuh"
 #include "mask_target.cuh"
+#include "launch_util.h"
 
 namespace mnc {
 namespace {
 
 constexpr int kRowThreads = 512;
 constexpr int kMaskThreads = 256;
-
-inline int check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 struct BridgeCfg {
   double mean[4], std_[4];

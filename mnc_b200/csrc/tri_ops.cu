@@ -5,11 +5,10 @@
 #include <cstdint>
 
 #include "mnc_b200.h"
+#include "launch_util.h"
 #include "tri.cuh"
 
 namespace mnc {
-
-static inline int tri_check_launch() { return cudaGetLastError() == cudaSuccess ? MNC_OK : MNC_ERR_CUDA; }
 
 __device__ __forceinline__ void amax_publish(float amx, unsigned int* amax) {
   if (amax == nullptr) return;
@@ -107,13 +106,6 @@ mask_pool_tri_kernel(const __half* __restrict__ f_h, const uint8_t* __restrict__
   }
 }
 
-static inline int tri_grid(long long n, int block) {
-  long long g = (n + block - 1) / block;
-  if (g > 132 * 16) g = 132 * 16;
-  if (g < 1) g = 1;
-  return static_cast<int>(g);
-}
-
 }  // namespace mnc
 
 using namespace mnc;
@@ -124,18 +116,18 @@ extern "C" int mnc_f32_to_tri(const float* in, long long n, float scale, void* h
   if (n % 4 != 0 || (reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(h) |
                       reinterpret_cast<uintptr_t>(l) | reinterpret_cast<uintptr_t>(c)) % 8 != 0)
     return MNC_ERR_ARG;
-  f32_to_tri_kernel<<<tri_grid(n / 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  f32_to_tri_kernel<<<grid_for(n / 4, 256, 132 * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       in, n / 4, scale, static_cast<__half*>(h), static_cast<uint8_t*>(l), static_cast<uint8_t*>(c), amax);
-  return tri_check_launch();
+  return check_launch();
 }
 
 extern "C" int mnc_tri_to_f32(const void* h, const void* l, long long n, float inv_scale, float* out,
                               void* stream) {
   if (n <= 0) return MNC_OK;
   if (n % 4 != 0 || (reinterpret_cast<uintptr_t>(out) % 16) != 0) return MNC_ERR_ARG;
-  tri_to_f32_kernel<<<tri_grid(n / 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  tri_to_f32_kernel<<<grid_for(n / 4, 256, 132 * 16), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __half*>(h), static_cast<const uint8_t*>(l), n / 4, inv_scale, out);
-  return tri_check_launch();
+  return check_launch();
 }
 
 extern "C" int mnc_splitk_reduce_tri(const float* partial, int splits, long long split_stride,
@@ -148,10 +140,11 @@ extern "C" int mnc_splitk_reduce_tri(const float* partial, int splits, long long
       reinterpret_cast<uintptr_t>(partial) % 16 != 0 ||
       (bias != nullptr && reinterpret_cast<uintptr_t>(bias) % 16 != 0) || !tri_planes_aligned(h, l, c))
     return MNC_ERR_ARG;
-  splitk_reduce_tri_kernel<<<tri_grid(rows * (cols / 4), 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+  splitk_reduce_tri_kernel<<<grid_for(rows * (cols / 4), 256, 132 * 16), 256, 0,
+                             static_cast<cudaStream_t>(stream)>>>(
       partial, splits, split_stride, rows, cols, bias, relu, scale, static_cast<__half*>(h),
       static_cast<uint8_t*>(l), static_cast<uint8_t*>(c), out_row_stride, out_ch_offset, amax);
-  return tri_check_launch();
+  return check_launch();
 }
 
 extern "C" int mnc_mask_pool_tri(const void* f_h, const void* f_l, const float* mask14, int R, int C,
@@ -163,5 +156,5 @@ extern "C" int mnc_mask_pool_tri(const void* f_h, const void* f_l, const float* 
   mask_pool_tri_kernel<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __half*>(f_h), static_cast<const uint8_t*>(f_l), mask14, C,
       static_cast<__half*>(o_h), static_cast<uint8_t*>(o_l), static_cast<uint8_t*>(o_c));
-  return tri_check_launch();
+  return check_launch();
 }
