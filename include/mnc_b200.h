@@ -545,6 +545,45 @@ int mnc_accuracy(const float* scores, const float* labels, int outer, int channe
                  const int* n_valid, int top_k, int has_ignore, int ignore_label, float* accuracy,
                  void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Head layers of the training net (InnerProduct, max Pooling, ReLU, Sigmoid), fp32 device blobs
+ * in Caffe layout; stream-ordered, no host synchronisation, no atomics, deterministic
+ * (DESIGN.md "Head layers for training").
+ *
+ * mnc_fc_forward: inner_product_layer.cu:9-27.  x (M, K) with K in Caffe's (c, h, w) order,
+ * w (N, K), b (N) or NULL (bias_term false), y (M, N) = x w^T, then + b in float32.  The product is
+ * split-bf16 on the tensor cores (hi*hi + hi*lo + lo*hi, float32 accumulators).
+ * mnc_fc_backward: inner_product_layer.cu:29-55.  dw (N, K) += dy^T x and db (N) += sum_m dy[m, :]
+ * (m ascending) accumulate, as Caffe's shared parameters rely on; dx (M, K) = dy w is overwritten.
+ * A NULL dw / db / dx is neither computed nor touched.
+ * Both take a workspace of mnc_fc_workspace_bytes(M, N, K) bytes (NULL when that is 0) for the
+ * split-K partials, which are added in split order; mnc_fc_split_k(rows, cols, red) is the split
+ * count of one (rows x cols) product reduced over red (pure host function of the shape). */
+int mnc_fc_split_k(int rows, int cols, int red);
+long long mnc_fc_workspace_bytes(int M, int N, int K);
+int mnc_fc_forward(const float* x, const float* w, const float* b, float* y, int M, int N, int K,
+                   void* workspace, long long workspace_bytes, void* stream);
+int mnc_fc_backward(const float* x, const float* w, const float* dy, float* dx, float* dw,
+                    float* db, int M, int N, int K, void* workspace, long long workspace_bytes,
+                    void* stream);
+
+/* mnc_max_pool_nchw: pooling_layer.cu:9-44 (MaxPoolForward), output (N, C, PH, PW) with
+ * PH = ceil((H - kernel) / stride) + 1 (pooling_layer.cpp:90-100); mask int32 holds h * W + w of
+ * the first maximum in row-major order (-FLT_MAX and -1 for a window of NaNs).  Only kernel 2,
+ * stride 2, pad 0 (the nets' head pools) is supported; anything else is MNC_ERR_ARG.
+ * mnc_max_pool_backward_nchw: MaxPoolBackward (pooling_layer.cu), dx (N, C, H, W) written whole. */
+int mnc_max_pool_nchw(const float* x, int N, int C, int H, int W, int kernel, int stride, int pad,
+                      float* y, int* mask, void* stream);
+int mnc_max_pool_backward_nchw(const float* dy, const int* mask, int N, int C, int H, int W,
+                               int kernel, int stride, int pad, float* dx, void* stream);
+/* mnc_relu / mnc_relu_backward: relu_layer.cu:9-41 with negative_slope 0: y = x > 0 ? x : x * 0,
+ * dx = dy * ((x > 0) + (x <= 0) * 0).  mnc_sigmoid / mnc_sigmoid_backward: sigmoid_layer.cu:10-40,
+ * dx = (dy * y) * (1 - y) from the forward's output y.  n elements. */
+int mnc_relu(const float* x, long long n, float* y, void* stream);
+int mnc_relu_backward(const float* x, const float* dy, long long n, float* dx, void* stream);
+int mnc_sigmoid(const float* x, long long n, float* y, void* stream);
+int mnc_sigmoid_backward(const float* y, const float* dy, long long n, float* dx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -327,3 +327,87 @@ def accuracy(scores, labels, top_k=1, ignore_label=None, n_valid=None):
     """Accuracy (ops.accuracy); not differentiable.  The training net sets no ignore label."""
     with torch.no_grad():
         return ops.accuracy(scores.detach(), labels.detach(), top_k, ignore_label, n_valid)
+
+
+# ------------------------------------------------------------------ training-net head layers
+class _InnerProduct(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b):
+        x, w = _c(x), _c(w)
+        b = None if b is None else _c(b)
+        ctx.save_for_backward(x, w)
+        ctx.x_shape, ctx.has_b = x.shape, b is not None
+        return ops.fc_forward(x, w, b)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, w = ctx.saved_tensors
+        want_x, want_w, want_b = ctx.needs_input_grad
+        dw = torch.zeros_like(w) if want_w else None
+        db = torch.zeros(w.shape[0], dtype=torch.float32, device=w.device) \
+            if want_b and ctx.has_b else None
+        dx = ops.fc_backward(x, w, _c(grad), dw=dw, db=db, want_dx=want_x)
+        return (None if dx is None else dx.view(ctx.x_shape)), dw, db
+
+
+class _MaxPool(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        x = _c(x)
+        y, mask = ops.max_pool_nchw(x)
+        ctx.save_for_backward(mask)
+        ctx.in_shape = x.shape
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        mask, = ctx.saved_tensors
+        return ops.max_pool_backward_nchw(_c(grad), mask, ctx.in_shape)
+
+
+class _ReLU(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        x = _c(x)
+        ctx.save_for_backward(x)
+        return ops.relu(x)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, = ctx.saved_tensors
+        return ops.relu_backward(x, _c(grad))
+
+
+class _Sigmoid(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        y = ops.sigmoid(_c(x))
+        ctx.save_for_backward(y)
+        return y
+
+    @staticmethod
+    def backward(ctx, grad):
+        y, = ctx.saved_tensors
+        return ops.sigmoid_backward(y, _c(grad))
+
+
+def inner_product(x, w, b=None):
+    """InnerProduct (ops.fc_forward): x (M, ...) -> (M, N).  Out of place: each use returns its own
+    gradients for w and b; a parameter shared by two uses (fc6 and fc6_ext, ...) gets the sum of
+    the two from autograd, as Caffe's shared blobs accumulate it."""
+    return _InnerProduct.apply(x, w, b)
+
+
+def max_pool(x):
+    """Pooling MAX, kernel 2, stride 2, pad 0 (ops.max_pool_nchw): (N,C,H,W) -> ceil-mode halves."""
+    return _MaxPool.apply(x)
+
+
+def relu(x):
+    """ReLU, negative_slope 0 (ops.relu)."""
+    return _ReLU.apply(x)
+
+
+def sigmoid(x):
+    """Sigmoid (ops.sigmoid)."""
+    return _Sigmoid.apply(x)

@@ -19,6 +19,7 @@
 
 #include "mnc_b200.h"
 #include "launch_util.h"
+#include "sigmoid.cuh"
 
 namespace mnc {
 namespace {
@@ -222,12 +223,6 @@ smooth_l1_loss_backward_kernel(const float* __restrict__ b0, const float* __rest
 }
 
 // ------------------------------------------------------------------ SigmoidCrossEntropyLoss
-// SigmoidForward (sigmoid_layer.cu:9-14) as the reference build compiles it: expf of the float
-// argument, then 1 + e and the quotient in double, rounded to float once.
-__device__ __forceinline__ float ref_sigmoid(float x) {
-  return static_cast<float>(__ddiv_rn(1.0, __dadd_rn(1.0, static_cast<double>(expf(-x)))));
-}
-
 // One term of sigmoid_cross_entropy_loss_layer.cpp:44-58 as the reference's object evaluates it:
 // <math.h> (through mkl_alternate.hpp) puts the float overloads of exp / log in scope, so the
 // whole term is float -- expf, 1 + e, logf, a - l, w * (...) -- each operation rounded.

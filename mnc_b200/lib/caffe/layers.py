@@ -331,3 +331,118 @@ class AccuracyLayer(_NativeLayer):
         if any(propagate_down):
             raise NotImplementedError("NOT_IMPLEMENTED (as in the reference)")
 
+
+
+# ------------------------------------------------------------------ head layers of the training net
+class InnerProductLayer(_NativeLayer):
+    """inner_product_layer.cpp:10-87 (setup / reshape, axis 1), inner_product_layer.cu:9-55.
+    blobs_ = [W (N, K), b (N)]; set their data before the first Forward.  Backward ADDS to the
+    blobs' diffs (beta 1), so a layer given another layer's blobs_ (fc6_ext sharing fc6's) sums the
+    two uses' gradients, as Caffe's shared parameters do; the solver zeroes them per step."""
+
+    def LayerSetUp(self, bottom, top):
+        from mnc_b200.lib.caffe import Blob
+        p = self.layer_param_.get("inner_product_param", {})
+        if int(p.get("axis", 1)) != 1:
+            raise ValueError("InnerProduct: only axis 1 is supported")
+        if p.get("transpose", False):
+            raise ValueError("InnerProduct: transpose is not supported")
+        self.N_ = int(p["num_output"])
+        self.bias_term_ = bool(p.get("bias_term", True))
+        self.K_ = bottom[0].count // bottom[0].num
+        self.blobs_ = [Blob(self.N_, self.K_)] + ([Blob(self.N_)] if self.bias_term_ else [])
+        self.param_propagate_down_ = [True] * len(self.blobs_)
+
+    def Reshape(self, bottom, top):
+        if bottom[0].count // bottom[0].num != self.K_:
+            raise ValueError("Input size incompatible with inner product parameters.")
+        top[0].reshape(bottom[0].num, self.N_)
+
+    def _params(self):
+        w = _dev(self.blobs_[0].data)
+        b = _dev(self.blobs_[1].data) if self.bias_term_ else None
+        return w, b
+
+    def Forward_gpu(self, bottom, top):
+        w, b = self._params()
+        top[0].data[...] = ops.fc_forward(_dev(bottom[0].data), w, b).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        w, _ = self._params()
+        want_w = self.param_propagate_down_[0]
+        want_b = self.bias_term_ and self.param_propagate_down_[1]
+        want_x = bool(propagate_down[0])
+        dw = _dev(_diff(self.blobs_[0])) if want_w else None
+        db = _dev(_diff(self.blobs_[1])) if want_b else None
+        if not (want_w or want_b or want_x):
+            return
+        dx = ops.fc_backward(_dev(bottom[0].data), w, _dev(top[0].diff), dw=dw, db=db,
+                             want_dx=want_x)
+        if want_w:
+            self.blobs_[0].diff[...] = dw.cpu().numpy()
+        if want_b:
+            self.blobs_[1].diff[...] = db.cpu().numpy()
+        if want_x:
+            _diff(bottom[0])[...] = dx.cpu().numpy().reshape(bottom[0].shape)
+
+
+class PoolingLayer(_NativeLayer):
+    """pooling_layer.cpp:12-100 (setup / reshape), pooling_layer.cu MaxPoolForward /
+    MaxPoolBackward; MAX only, kernel 2, stride 2, pad 0 (the head pools of the nets)."""
+
+    def LayerSetUp(self, bottom, top):
+        p = self.layer_param_.get("pooling_param", {})
+        ok = (p.get("pool", "MAX") in ("MAX", 0) and int(p.get("kernel_size", 0)) == 2 and
+              int(p.get("stride", 1)) == 2 and int(p.get("pad", 0)) == 0 and
+              not p.get("global_pooling", False))
+        if not ok:
+            raise ValueError("Pooling: only MAX with kernel_size 2, stride 2, pad 0 is supported")
+
+    def Reshape(self, bottom, top):
+        b = bottom[0]
+        top[0].reshape(b.num, b.channels, ops._pool_out(b.height), ops._pool_out(b.width))
+
+    def Forward_gpu(self, bottom, top):
+        y, self.max_idx_ = ops.max_pool_nchw(_dev(bottom[0].data))
+        top[0].data[...] = y.cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        """pooling_layer.cu: nothing is written unless propagated."""
+        if not propagate_down[0]:
+            return
+        _diff(bottom[0])[...] = ops.max_pool_backward_nchw(
+            _dev(top[0].diff), self.max_idx_, bottom[0].shape).cpu().numpy()
+
+
+class ReLULayer(_NativeLayer):
+    """relu_layer.cu:9-41, negative_slope 0 (the nets' ReLUs)."""
+
+    def LayerSetUp(self, bottom, top):
+        if float(self.layer_param_.get("relu_param", {}).get("negative_slope", 0.0)) != 0.0:
+            raise ValueError("ReLU: only negative_slope 0 is supported")
+
+    def Reshape(self, bottom, top):
+        top[0].reshape(*bottom[0].shape)
+
+    def Forward_gpu(self, bottom, top):
+        top[0].data[...] = ops.relu(_dev(bottom[0].data)).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        if propagate_down[0]:
+            _diff(bottom[0])[...] = ops.relu_backward(_dev(bottom[0].data),
+                                                      _dev(top[0].diff)).cpu().numpy()
+
+
+class SigmoidLayer(_NativeLayer):
+    """sigmoid_layer.cu:10-40; the backward reads the top's data."""
+
+    def Reshape(self, bottom, top):
+        top[0].reshape(*bottom[0].shape)
+
+    def Forward_gpu(self, bottom, top):
+        top[0].data[...] = ops.sigmoid(_dev(bottom[0].data)).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        if propagate_down[0]:
+            _diff(bottom[0])[...] = ops.sigmoid_backward(_dev(top[0].data),
+                                                         _dev(top[0].diff)).cpu().numpy()

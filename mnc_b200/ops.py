@@ -890,3 +890,127 @@ def accuracy(scores, labels, top_k=1, ignore_label=None, n_valid=None):
                            top_k, int(ignore_label is not None), int(ignore_label or 0), ptr(out),
                            cur_stream()), "mnc_accuracy")
     return out
+
+
+# ----------------------------------------------------------------------------- head layers (training)
+def _fc_workspace(M, N, K, device):
+    n = lib.mnc_fc_workspace_bytes(M, N, K)
+    return torch.empty(n, dtype=torch.uint8, device=device) if n else None
+
+
+def _fc_launches(rows, cols, red):
+    """Kernels of one product: the GEMM, plus the split-K reduction when it splits."""
+    return 1 if lib.mnc_fc_split_k(rows, cols, red) == 1 else 2
+
+
+def _fc_shape(x, w):
+    N, K = w.shape
+    M = x.shape[0]
+    if x.numel() != M * K:
+        raise ValueError("InnerProduct: bottom count %d is not %d x %d" % (x.numel(), M, K))
+    return M, N, K
+
+
+def fc_forward(x, w, b=None):
+    """InnerProduct forward (inner_product_layer.cu:9-27): x (M, ...) flattened to (M, K),
+    w (N, K), b (N) or None -> y (M, N) = x w^T + b, split-bf16 on the tensor cores."""
+    x, w = _f32(x), _f32(w)
+    M, N, K = _fc_shape(x, w)
+    b = None if b is None else _f32(b)
+    y = torch.empty((M, N), dtype=torch.float32, device=x.device)
+    ws = _fc_workspace(M, N, K, x.device)
+    check(lib.mnc_fc_forward(ptr(x), ptr(w), ptr(b), ptr(y), M, N, K, ptr(ws),
+                             0 if ws is None else ws.numel(), cur_stream()),
+          "mnc_fc_forward", launches=_fc_launches(N, M, K))
+    return y
+
+
+def fc_backward(x, w, dy, dw=None, db=None, want_dx=True):
+    """InnerProduct backward (inner_product_layer.cu:29-55).  dw (N, K) and db (N), when given,
+    are contiguous float32 tensors the gradients are ADDED to (beta 1); -> dx (M, K), overwritten
+    (beta 0), or None when not wanted."""
+    x, w, dy = _f32(x), _f32(w), _f32(dy)
+    M, N, K = _fc_shape(x, w)
+    if dy.numel() != M * N:
+        raise ValueError("InnerProduct: top diff count %d is not %d x %d" % (dy.numel(), M, N))
+    for t, n in ((dw, N * K), (db, N)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n):
+            raise ValueError("InnerProduct: parameter diffs must be contiguous float32 of the "
+                             "parameter's size")
+    dx = torch.empty((M, K), dtype=torch.float32, device=x.device) if want_dx else None
+    ws = _fc_workspace(M, N, K, x.device)
+    launches = (_fc_launches(N, K, M) if dw is not None else 0) + (db is not None) + \
+        (_fc_launches(K, M, N) if want_dx else 0)
+    check(lib.mnc_fc_backward(ptr(x), ptr(w), ptr(dy), ptr(dx), ptr(dw), ptr(db), M, N, K,
+                              ptr(ws), 0 if ws is None else ws.numel(), cur_stream()),
+          "mnc_fc_backward", launches=launches)
+    return dx
+
+
+def _pool_out(h):
+    """pooling_layer.cpp:90-100 at kernel 2, stride 2, pad 0 (ceil mode)."""
+    return (max(h - 2, 0) + 1) // 2 + 1
+
+
+def max_pool_nchw(x):
+    """Pooling MAX, kernel 2, stride 2, pad 0 (pooling_layer.cu:9-44): x (N, C, H, W) ->
+    (y (N, C, ceil((H-2)/2)+1, ...), mask int32 of the same shape)."""
+    x = _f32(x)
+    N, C, H, W = x.shape
+    shape = (N, C, _pool_out(H), _pool_out(W))
+    y = torch.empty(shape, dtype=torch.float32, device=x.device)
+    mask = torch.empty(shape, dtype=torch.int32, device=x.device)
+    check(lib.mnc_max_pool_nchw(ptr(x), N, C, H, W, 2, 2, 0, ptr(y), ptr(mask), cur_stream()),
+          "mnc_max_pool_nchw")
+    return y, mask
+
+
+def max_pool_backward_nchw(dy, mask, in_shape):
+    """MaxPoolBackward: -> dx of shape in_shape (N, C, H, W), written whole."""
+    dy, mask = _f32(dy), mask.contiguous()
+    N, C, H, W = in_shape
+    if tuple(dy.shape) != (N, C, _pool_out(H), _pool_out(W)) or mask.shape != dy.shape or \
+            mask.dtype != torch.int32:
+        raise ValueError("max_pool_backward_nchw: dy / mask do not match the pooled shape")
+    dx = torch.empty(tuple(in_shape), dtype=torch.float32, device=dy.device)
+    check(lib.mnc_max_pool_backward_nchw(ptr(dy), ptr(mask), N, C, H, W, 2, 2, 0, ptr(dx),
+                                         cur_stream()), "mnc_max_pool_backward_nchw")
+    return dx
+
+
+def relu(x):
+    """ReLU, negative_slope 0 (relu_layer.cu:9-14): x > 0 ? x : x * 0."""
+    x = _f32(x)
+    y = torch.empty_like(x)
+    check(lib.mnc_relu(ptr(x), x.numel(), ptr(y), cur_stream()), "mnc_relu")
+    return y
+
+
+def relu_backward(x, dy):
+    """ReLU backward (relu_layer.cu:27-33): dy * ((x > 0) + (x <= 0) * 0)."""
+    x, dy = _f32(x), _f32(dy)
+    if dy.numel() != x.numel():
+        raise ValueError("relu_backward: x and dy must have the same count")
+    dx = torch.empty_like(x)
+    check(lib.mnc_relu_backward(ptr(x), ptr(dy), x.numel(), ptr(dx), cur_stream()),
+          "mnc_relu_backward")
+    return dx
+
+
+def sigmoid(x):
+    """Sigmoid (sigmoid_layer.cu:9-21), the reference build's arithmetic (DESIGN.md)."""
+    x = _f32(x)
+    y = torch.empty_like(x)
+    check(lib.mnc_sigmoid(ptr(x), x.numel(), ptr(y), cur_stream()), "mnc_sigmoid")
+    return y
+
+
+def sigmoid_backward(y, dy):
+    """Sigmoid backward (sigmoid_layer.cu:23-40) from the forward's output: (dy * y) * (1 - y)."""
+    y, dy = _f32(y), _f32(dy)
+    if dy.numel() != y.numel():
+        raise ValueError("sigmoid_backward: y and dy must have the same count")
+    dx = torch.empty_like(y)
+    check(lib.mnc_sigmoid_backward(ptr(y), ptr(dy), y.numel(), ptr(dx), cur_stream()),
+          "mnc_sigmoid_backward")
+    return dx
