@@ -584,6 +584,34 @@ int mnc_relu_backward(const float* x, const float* dy, long long n, float* dx, v
 int mnc_sigmoid(const float* x, long long n, float* y, void* stream);
 int mnc_sigmoid_backward(const float* y, const float* dy, long long n, float* dx, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Convolution of the training net (the VGG-16 trunk and the RPN), fp32 NCHW device blobs in Caffe
+ * layout; stream-ordered, no host synchronisation, no atomics, deterministic (DESIGN.md "Trunk and
+ * RPN convolutions for training").
+ *
+ * mnc_conv_forward: conv_layer.cu:10-24 with base_conv_layer.cpp:232-257 (im2col + sgemm per image,
+ * then the bias).  x (N, Cin, H, W), w (Cout, Cin, kernel, kernel), b (Cout) or NULL (bias_term
+ * false), y (N, Cout, H, W) = conv(x, w) + b in float32.  Only kernel 3 / pad 1 and kernel 1 /
+ * pad 0, both at stride 1, are supported (dilation 1, group 1); anything else is MNC_ERR_ARG.
+ * The products are split-bf16 on the tensor cores, the InnerProduct GEMM with the image operand
+ * gathered (zero padding) in its loader: no column buffer.
+ * mnc_conv_backward: conv_layer.cu:26-62 with base_conv_layer.cpp:259-294.  dw (Cout, Cin, k, k)
+ * += sum over images of dy (x) and db (Cout) += sum of dy over pixels, then images, accumulate
+ * (beta 1); dx (N, Cin, H, W) is overwritten.  A NULL dw / db / dx is neither computed nor touched.
+ * mnc_conv_backward takes a workspace of mnc_conv_workspace_bytes(N, Cin, H, W, Cout, kernel) bytes
+ * (NULL when that is 0); a shorter one is MNC_ERR_ARG.  It holds the split-K partials of the
+ * largest per-image product (split count mnc_fc_split_k) and, for kernel 3, dx's transposed weight
+ * after them.  mnc_conv_forward uses only the partials of its own product: it needs
+ * s * Cout * H * W * 4 bytes with s = mnc_fc_split_k(Cout, H * W, Cin * kernel * kernel) when s > 1,
+ * none otherwise; a workspace of mnc_conv_workspace_bytes serves both calls. */
+long long mnc_conv_workspace_bytes(int N, int Cin, int H, int W, int Cout, int kernel);
+int mnc_conv_forward(const float* x, const float* w, const float* b, float* y, int N, int Cin,
+                     int H, int W, int Cout, int kernel, int pad, int stride, void* workspace,
+                     long long workspace_bytes, void* stream);
+int mnc_conv_backward(const float* x, const float* w, const float* dy, float* dx, float* dw,
+                      float* db, int N, int Cin, int H, int W, int Cout, int kernel, int pad,
+                      int stride, void* workspace, long long workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

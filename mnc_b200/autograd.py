@@ -350,6 +350,26 @@ class _InnerProduct(torch.autograd.Function):
         return (None if dx is None else dx.view(ctx.x_shape)), dw, db
 
 
+class _Convolution(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b):
+        x, w = _c(x), _c(w)
+        b = None if b is None else _c(b)
+        ctx.save_for_backward(x, w)
+        ctx.has_b = b is not None
+        return ops.conv_forward(x, w, b)
+
+    @staticmethod
+    def backward(ctx, grad):
+        x, w = ctx.saved_tensors
+        want_x, want_w, want_b = ctx.needs_input_grad
+        dw = torch.zeros_like(w) if want_w else None
+        db = torch.zeros(w.shape[0], dtype=torch.float32, device=w.device) \
+            if want_b and ctx.has_b else None
+        dx = ops.conv_backward(x, w, _c(grad), dw=dw, db=db, want_dx=want_x)
+        return dx, dw, db
+
+
 class _MaxPool(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x):
@@ -396,6 +416,13 @@ def inner_product(x, w, b=None):
     gradients for w and b; a parameter shared by two uses (fc6 and fc6_ext, ...) gets the sum of
     the two from autograd, as Caffe's shared blobs accumulate it."""
     return _InnerProduct.apply(x, w, b)
+
+
+def convolution(x, w, b=None):
+    """Convolution, stride 1 (ops.conv_forward): x (N, Cin, H, W), w (Cout, Cin, k, k) with k 3
+    (pad 1) or 1 (pad 0) -> (N, Cout, H, W).  Out of place, as inner_product: a parameter shared or
+    used twice gets the sum of its uses' gradients from autograd."""
+    return _Convolution.apply(x, w, b)
 
 
 def max_pool(x):

@@ -446,3 +446,78 @@ class SigmoidLayer(_NativeLayer):
         if propagate_down[0]:
             _diff(bottom[0])[...] = ops.sigmoid_backward(_dev(top[0].data),
                                                          _dev(top[0].diff)).cpu().numpy()
+
+
+def _conv_field(p, name, default):
+    """A repeated uint field of convolution_param (kernel_size, pad, stride, dilation) as one value:
+    a single entry, or several equal ones; unequal entries (a non-square form) raise."""
+    v = p.get(name, default)
+    vals = [int(u) for u in v] if isinstance(v, (list, tuple)) else [int(v)]
+    if not vals:
+        vals = [default]
+    if len(set(vals)) != 1:
+        raise ValueError("Convolution: only square %s is supported" % name)
+    return vals[0]
+
+
+class ConvolutionLayer(_NativeLayer):
+    """base_conv_layer.cpp:12-186 (setup / reshape), conv_layer.cu:10-62; stride 1 with kernel 3 /
+    pad 1 or kernel 1 / pad 0, dilation 1, group 1 (the trunk and RPN convolutions of the nets).
+    blobs_ = [W (Cout, Cin, k, k), b (Cout)]; set their data before the first Forward.  Backward
+    ADDS to the blobs' diffs (beta 1) and honours param_propagate_down_ (False for a frozen,
+    lr_mult 0, layer: its diffs are neither computed nor touched) and propagate_down."""
+
+    def LayerSetUp(self, bottom, top):
+        from mnc_b200.lib.caffe import Blob
+        p = self.layer_param_.get("convolution_param", {})
+        for hw in ("kernel_h", "kernel_w", "pad_h", "pad_w", "stride_h", "stride_w"):
+            if hw in p:
+                raise ValueError("Convolution: %s is not supported" % hw)
+        k = _conv_field(p, "kernel_size", 0)
+        pad = _conv_field(p, "pad", 0)
+        stride = _conv_field(p, "stride", 1)
+        dilation = _conv_field(p, "dilation", 1)
+        if not (stride == 1 and dilation == 1 and int(p.get("group", 1)) == 1 and
+                int(p.get("axis", 1)) == 1 and (k, pad) in ((3, 1), (1, 0))):
+            raise ValueError("Convolution: only kernel 3 / pad 1 or kernel 1 / pad 0 at stride 1, "
+                             "dilation 1, group 1 is supported")
+        self.k_, self.pad_ = k, pad
+        self.num_output_ = int(p["num_output"])
+        self.bias_term_ = bool(p.get("bias_term", True))
+        self.channels_ = bottom[0].channels
+        self.blobs_ = [Blob(self.num_output_, self.channels_, k, k)] + \
+            ([Blob(self.num_output_)] if self.bias_term_ else [])
+        self.param_propagate_down_ = [True] * len(self.blobs_)
+
+    def Reshape(self, bottom, top):
+        b = bottom[0]
+        if b.channels != self.channels_:
+            raise ValueError("Input size incompatible with convolution kernel.")
+        top[0].reshape(b.num, self.num_output_, b.height, b.width)
+
+    def _params(self):
+        w = _dev(self.blobs_[0].data)
+        b = _dev(self.blobs_[1].data) if self.bias_term_ else None
+        return w, b
+
+    def Forward_gpu(self, bottom, top):
+        w, b = self._params()
+        top[0].data[...] = ops.conv_forward(_dev(bottom[0].data), w, b, pad=self.pad_).cpu().numpy()
+
+    def Backward_gpu(self, top, propagate_down, bottom):
+        w, _ = self._params()
+        want_w = self.param_propagate_down_[0]
+        want_b = self.bias_term_ and self.param_propagate_down_[1]
+        want_x = bool(propagate_down[0])
+        if not (want_w or want_b or want_x):
+            return
+        dw = _dev(_diff(self.blobs_[0])) if want_w else None
+        db = _dev(_diff(self.blobs_[1])) if want_b else None
+        dx = ops.conv_backward(_dev(bottom[0].data), w, _dev(top[0].diff), dw=dw, db=db,
+                               want_dx=want_x)
+        if want_w:
+            self.blobs_[0].diff[...] = dw.cpu().numpy()
+        if want_b:
+            self.blobs_[1].diff[...] = db.cpu().numpy()
+        if want_x:
+            _diff(bottom[0])[...] = dx.cpu().numpy()

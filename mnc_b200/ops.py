@@ -1014,3 +1014,69 @@ def sigmoid_backward(y, dy):
     check(lib.mnc_sigmoid_backward(ptr(y), ptr(dy), y.numel(), ptr(dx), cur_stream()),
           "mnc_sigmoid_backward")
     return dx
+
+
+# ----------------------------------------------------------------------------- convolution (training)
+def _conv_shape(x, w, *others):
+    """(N, Cin, H, W, Cout, k) of x (N, Cin, H, W) and w (Cout, Cin, k, k); x, w and the tensors
+    in `others` (None skipped) must be CUDA tensors on one device."""
+    if x.dim() != 4 or w.dim() != 4 or w.shape[2] != w.shape[3]:
+        raise ValueError("Convolution: x must be (N, C, H, W) and w (Cout, Cin, k, k)")
+    N, Cin, H, W = x.shape
+    Cout, wc, k, _ = w.shape
+    if wc != Cin:
+        raise ValueError("Convolution: w has %d input channels, x has %d" % (wc, Cin))
+    devs = {t.device for t in (x, w) + others if t is not None}
+    if len(devs) != 1 or next(iter(devs)).type != "cuda":
+        raise ValueError("Convolution: all tensors must be on one CUDA device, got %s" % sorted(map(str, devs)))
+    return N, Cin, H, W, Cout, k
+
+
+def _conv_workspace(N, Cin, H, W, Cout, k, device):
+    n = lib.mnc_conv_workspace_bytes(N, Cin, H, W, Cout, k)
+    return torch.empty(n, dtype=torch.uint8, device=device) if n else None
+
+
+def conv_forward(x, w, b=None, pad=None):
+    """Convolution forward (conv_layer.cu:10-24), stride 1: x (N, Cin, H, W), w (Cout, Cin, k, k),
+    b (Cout) or None -> y (N, Cout, H, W), split-bf16 on the tensor cores.  k 3 with pad 1 or k 1
+    with pad 0 (pad None: (k - 1) / 2); anything else raises."""
+    x, w = _f32(x), _f32(w)
+    b = None if b is None else _f32(b)
+    N, Cin, H, W, Cout, k = _conv_shape(x, w, b)
+    if b is not None and b.numel() != Cout:
+        raise ValueError("Convolution: bias has %d elements, not Cout = %d" % (b.numel(), Cout))
+    pad = (k - 1) // 2 if pad is None else pad
+    y = torch.empty((N, Cout, H, W), dtype=torch.float32, device=x.device)
+    # only the split-K partials of the forward product (include/mnc_b200.h)
+    s = lib.mnc_fc_split_k(Cout, H * W, Cin * k * k)
+    ws = torch.empty(s * Cout * H * W * 4, dtype=torch.uint8, device=x.device) if s > 1 else None
+    check(lib.mnc_conv_forward(ptr(x), ptr(w), ptr(b), ptr(y), N, Cin, H, W, Cout, k, pad, 1,
+                               ptr(ws), 0 if ws is None else ws.numel(), cur_stream()),
+          "mnc_conv_forward", launches=N * _fc_launches(Cout, H * W, Cin * k * k))
+    return y
+
+
+def conv_backward(x, w, dy, dw=None, db=None, want_dx=True):
+    """Convolution backward (conv_layer.cu:26-62), stride 1, pad (k - 1) / 2.  dw (Cout, Cin, k, k)
+    and db (Cout), when given, are contiguous float32 tensors the gradients are ADDED to (beta 1);
+    -> dx (N, Cin, H, W), overwritten (beta 0), or None when not wanted."""
+    x, w, dy = _f32(x), _f32(w), _f32(dy)
+    N, Cin, H, W, Cout, k = _conv_shape(x, w, dy, dw, db)
+    if tuple(dy.shape) != (N, Cout, H, W):
+        raise ValueError("Convolution: top diff shape %s is not %s" % (tuple(dy.shape),
+                                                                       (N, Cout, H, W)))
+    for t, n in ((dw, Cout * Cin * k * k), (db, Cout)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != n):
+            raise ValueError("Convolution: parameter diffs must be contiguous float32 of the "
+                             "parameter's size")
+    dx = torch.empty((N, Cin, H, W), dtype=torch.float32, device=x.device) if want_dx else None
+    ws = _conv_workspace(N, Cin, H, W, Cout, k, x.device)
+    HW, taps = H * W, k * k
+    launches = (N * _fc_launches(Cout, Cin * taps, HW) if dw is not None else 0) + \
+        (db is not None) + (N * _fc_launches(Cin, HW, Cout * taps) + (k == 3) if want_dx else 0)
+    check(lib.mnc_conv_backward(ptr(x), ptr(w), ptr(dy), ptr(dx), ptr(dw), ptr(db), N, Cin, H, W,
+                                Cout, k, (k - 1) // 2, 1, ptr(ws), 0 if ws is None else ws.numel(),
+                                cur_stream()),
+          "mnc_conv_backward", launches=launches)
+    return dx

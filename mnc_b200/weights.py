@@ -18,6 +18,31 @@ TRUNK_NAMES = ["conv1_1", "conv1_2", "conv2_1", "conv2_2", "conv3_1", "conv3_2",
 POOL_AFTER = {"conv1_2", "conv2_2", "conv3_3", "conv4_3"}
 
 
+def _train_convs():
+    out, cin, level = [], 3, 0
+    for name, cout in zip(TRUNK_NAMES, FULL_ARCH["trunk"]):
+        out.append((name, cin, cout, 3, level, not name.startswith(("conv1", "conv2"))))
+        cin = cout
+        level += name in POOL_AFTER
+    r = FULL_ARCH["rpn"]
+    return out + [("rpn_conv_3x3", cin, r, 3, level, True), ("rpn_cls_score", r, 18, 1, level, True),
+                  ("rpn_bbox_pred", r, 36, 1, level, True)]
+
+
+# The 16 convolutions of models/VGG16/mnc_5stage/train.prototxt: (name, Cin, Cout, kernel, level,
+# learns), level = the number of 2x2 ceil-mode pools above the layer, learns = lr_mult > 0
+# (conv1_x and conv2_x are frozen)
+TRAIN_CONVS = _train_convs()
+
+
+def train_conv_size(H, W, level):
+    """Spatial size of a level of the trunk for an H x W image: `level` max pools of kernel 2,
+    stride 2, pad 0, ceil mode (pooling_layer.cpp:90-100)."""
+    for _ in range(level):
+        H, W = (max(H - 2, 0) + 1) // 2 + 1, (max(W - 2, 0) + 1) // 2 + 1
+    return H, W
+
+
 def make_weights(arch=None, seed=2016):
     """conv & FC weights N(0, sqrt(2/fan_in)), biases 0; RPN weights N(0, 0.01) as the prototxt
     fillers say.  conv1_1 is scaled by 1/64 (mean-subtracted pixels are ~70 RMS) so activations
