@@ -7,7 +7,7 @@
  * forward restatements.  Only tests/ and scripts/ load this library (via oracle/oracle_backward.py);
  * mnc_b200/ never does.  Each function cites the reference file:line it follows and mirrors its
  * expressions term by term (same int/float/double promotions), compiled with -ffp-contract=off.
- * Pinned against the reference's own Backward_gpu compiled unmodified (oracle/backward.mk,
+ * Pinned against the reference's own Backward_gpu compiled unmodified (oracle/Makefile,
  * tests/test_ref_pin_backward.py): bit-exact against the -fmad=false build for every feature and
  * mask gradient.
  */

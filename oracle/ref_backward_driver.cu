@@ -1,5 +1,5 @@
 // oracle/ref_backward_driver.cu -- TEST INFRASTRUCTURE.  C entry points that run the reference's
-// own layer objects (compiled unmodified from the reference checkout, see oracle/backward.mk) the
+// own layer objects (compiled unmodified from the reference checkout, see oracle/Makefile) the
 // way Caffe's Net does for a training step: construct from a LayerParameter, SetUp (LayerSetUp +
 // Reshape), Forward (Reshape + Forward_gpu), fill the top diff, then Backward (Backward_gpu) on the
 // same layer object, so the argmax / buffer blobs it reads are the layer's own.  Plain host

@@ -1,7 +1,7 @@
 // oracle/ref_conv_driver.cu -- TEST INFRASTRUCTURE.  A C entry point that runs the reference's
-// ConvolutionLayer, compiled UNMODIFIED from a reference checkout with its im2col (oracle/conv.mk),
-// as Caffe runs it in GPU mode: SetUp, the parameters written, Forward, the top diff written,
-// Backward on the same object.  Host arrays in and out.  No layer arithmetic here.
+// ConvolutionLayer, compiled UNMODIFIED from a reference checkout with its im2col
+// (oracle/Makefile), as Caffe runs it in GPU mode: SetUp, the parameters written, Forward, the top
+// diff written, Backward on the same object.  Host arrays in and out.  No layer arithmetic here.
 #include <vector>
 
 #include "caffe/layers/conv_layer.hpp"

@@ -1,7 +1,8 @@
 // oracle/ref_heads_driver.cu -- TEST INFRASTRUCTURE.  C entry points that run the reference's head
 // layers (InnerProduct, Pooling MAX, ReLU, Sigmoid), compiled UNMODIFIED from a reference checkout
-// (oracle/heads.mk), as Caffe runs them in GPU mode: SetUp, the parameters written, Forward, the top
-// diff written, Backward on the same object.  Host arrays in and out.  No layer arithmetic here.
+// (oracle/Makefile), as Caffe runs them in GPU mode: SetUp, the parameters written, Forward, the
+// top diff written, Backward on the same object.  Host arrays in and out.  No layer arithmetic
+// here.
 #include <vector>
 
 #include "caffe/layers/inner_product_layer.hpp"

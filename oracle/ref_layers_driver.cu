@@ -1,5 +1,5 @@
 // oracle/ref_layers_driver.cu -- TEST INFRASTRUCTURE.  C entry points that run the reference's own
-// layer objects (compiled unmodified from /root/reference, see oracle/Makefile `ref`) the way
+// layer objects (compiled unmodified from a reference checkout, see oracle/Makefile) the way
 // Caffe's Net does: construct from a LayerParameter, SetUp (LayerSetUp + Reshape), Forward
 // (Reshape + Forward_gpu / Forward_cpu).  Plain host pointers in and out; ctypes binds these in
 // tests/test_ref_pin.py.

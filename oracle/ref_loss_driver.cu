@@ -1,8 +1,9 @@
 // oracle/ref_loss_driver.cu -- TEST INFRASTRUCTURE.  C entry points that run the reference's loss
-// layers, compiled UNMODIFIED from a reference checkout (oracle/loss.mk), as Caffe runs them in GPU
-// mode: SetUp, Forward, the top diff filled with the loss weight (what Net::Backward finds there),
-// Backward on the same object.  Host arrays in and out; `ms` (may be NULL) receives the event time
-// of Forward + Backward, the reference's host round trips included.  No layer arithmetic here.
+// layers, compiled UNMODIFIED from a reference checkout (oracle/Makefile), as Caffe runs them in
+// GPU mode: SetUp, Forward, the top diff filled with the loss weight (what Net::Backward finds
+// there), Backward on the same object.  Host arrays in and out; `ms` (may be NULL) receives the
+// event time of Forward + Backward, the reference's host round trips included.  No layer
+// arithmetic here.
 #include <vector>
 
 #include "caffe/fast_rcnn_layers.hpp"

@@ -1,24 +1,25 @@
 // oracle/ref_stub -- TEST INFRASTRUCTURE.  A minimal stand-in for the parts of the Caffe runtime
-// that the reference's MNC layer sources touch, so that
-//   caffe-mnc/src/caffe/layers/{roi_warping,mask_resize,mask_pooling,roi_pooling}_layer.{cu,cpp}
-// and the class declarations in caffe-mnc/include/caffe/fast_rcnn_layers.hpp and
-// caffe-mnc/include/caffe/layers/mask_resize_layer.hpp compile UNMODIFIED from /root/reference into
-// oracle/_ref/libmnc_ref_layers.so (oracle/Makefile `ref`).  Nothing here restates reference
-// arithmetic: kernels, LayerSetUp and Reshape are the reference's own object code.
-// Stands in for caffe-mnc/include/caffe/common.hpp + util/device_alternate.hpp + glog.
+// that the reference's layer sources touch, so that they compile UNMODIFIED from a reference
+// checkout into the libraries under oracle/_ref/ (oracle/Makefile).  Nothing here restates
+// reference arithmetic: kernels, LayerSetUp and Reshape are the reference's own object code.
+// Stands in for caffe-mnc/include/caffe/common.hpp + util/device_alternate.hpp + glog, with the
+// cuBLAS handle the math helpers (math_functions.cu) use.
 #ifndef MNC_REF_STUB_COMMON_HPP_
 #define MNC_REF_STUB_COMMON_HPP_
+#include <cublas_v2.h>
 #include <cuda_runtime.h>
 
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <iostream>
+#include <memory>
 #include <sstream>
 #include <string>
 #include <vector>
 
 namespace caffe {
+using std::shared_ptr;
 using std::string;
 using std::vector;
 
@@ -52,6 +53,8 @@ struct Voidify { template <typename T> void operator&(const T&) {} };
 #define STUB_LOG_FATAL ::caffe::stub::Fatal(__FILE__, __LINE__, "").os
 #define LOG(sev) STUB_LOG_##sev
 #define NOT_IMPLEMENTED LOG(FATAL) << "Not Implemented Yet"
+#define DCHECK_GE(a, b) ::caffe::stub::Null()
+#define DCHECK_LT(a, b) ::caffe::stub::Null()
 
 #define CUDA_CHECK(condition)                                                   \
   do {                                                                          \
@@ -63,6 +66,15 @@ struct Voidify { template <typename T> void operator&(const T&) {} };
 #define CUDA_POST_KERNEL_CHECK CUDA_CHECK(cudaPeekAtLastError())
 
 namespace caffe {
+class Caffe {
+ public:
+  static cublasHandle_t cublas_handle() {
+    static cublasHandle_t h = 0;
+    if (!h) cublasCreate(&h);
+    return h;
+  }
+};
+
 const int CAFFE_CUDA_NUM_THREADS = 512;  // device_alternate.hpp value for __CUDA_ARCH__ >= 200
 inline int CAFFE_GET_BLOCKS(const int N) {
   return (N + CAFFE_CUDA_NUM_THREADS - 1) / CAFFE_CUDA_NUM_THREADS;

@@ -1,12 +1,25 @@
-// oracle/ref_stub -- TEST INFRASTRUCTURE.  Stand-in for caffe-mnc/include/caffe/layer.hpp: the
-// Layer<Dtype> base with the SetUp / Reshape / Forward protocol (layer.hpp:67-77, 446-470).
+// oracle/ref_stub -- TEST INFRASTRUCTURE.  Stand-in for caffe/layer.hpp (+ the LayerRegistry of
+// layer_factory.hpp) as Caffe runs in GPU mode, with the learnable parameters a layer owns
+// (blobs_, param_propagate_down_): SetUp = LayerSetUp, Reshape, SetLossWeights (layer.hpp:67-77,
+// 417-433); Forward = Reshape, Forward_gpu (:446-470), or Forward_cpu when the driver asks for the
+// CPU path; Backward = Backward_gpu (:472-487).  A layer without Forward_gpu / Backward_gpu falls
+// back to its _cpu form, as in Caffe.  LayerRegistry<Dtype>::CreateLayer is defined by the driver
+// that needs it (oracle/ref_loss_driver.cu).
 #ifndef MNC_REF_STUB_LAYER_HPP_
 #define MNC_REF_STUB_LAYER_HPP_
 #include "caffe/blob.hpp"
 #include "caffe/common.hpp"
 #include "caffe/proto/caffe.pb.h"
+#include "caffe/util/math_functions.hpp"
 
 namespace caffe {
+template <typename Dtype> class Layer;
+
+template <typename Dtype>
+struct LayerRegistry {
+  static shared_ptr<Layer<Dtype> > CreateLayer(const LayerParameter& param);
+};
+
 template <typename Dtype>
 class Layer {
  public:
@@ -15,15 +28,22 @@ class Layer {
   void SetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
     LayerSetUp(bottom, top);
     Reshape(bottom, top);
+    SetLossWeights(top);
   }
   virtual void LayerSetUp(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {}
   virtual void Reshape(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) = 0;
-  // Net::ForwardFromTo -> Layer::Forward: Reshape before every forward (layer.hpp:457), then the
-  // mode's Forward_*
-  void Forward(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top, bool gpu) {
+  Dtype Forward(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top,
+                bool gpu = true) {
     Reshape(bottom, top);
     if (gpu) Forward_gpu(bottom, top); else Forward_cpu(bottom, top);
+    return Dtype(0);
   }
+  void Backward(const vector<Blob<Dtype>*>& top, const vector<bool>& propagate_down,
+                const vector<Blob<Dtype>*>& bottom) {
+    Backward_gpu(top, propagate_down, bottom);
+  }
+  vector<shared_ptr<Blob<Dtype> > >& blobs() { return blobs_; }
+  const LayerParameter& layer_param() const { return layer_param_; }
   virtual inline const char* type() const { return ""; }
   virtual inline int ExactNumBottomBlobs() const { return -1; }
   virtual inline int MinBottomBlobs() const { return -1; }
@@ -31,11 +51,15 @@ class Layer {
   virtual inline int ExactNumTopBlobs() const { return -1; }
   virtual inline int MinTopBlobs() const { return -1; }
   virtual inline int MaxTopBlobs() const { return -1; }
+  virtual inline bool EqualNumBottomTopBlobs() const { return false; }
+  virtual inline bool AutoTopBlobs() const { return false; }
   virtual inline bool AllowForceBackward(const int bottom_index) const { return true; }
 
  protected:
   LayerParameter layer_param_;
   Phase phase_;
+  vector<shared_ptr<Blob<Dtype> > > blobs_;
+  vector<bool> param_propagate_down_;
   virtual void Forward_cpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) = 0;
   virtual void Forward_gpu(const vector<Blob<Dtype>*>& bottom, const vector<Blob<Dtype>*>& top) {
     Forward_cpu(bottom, top);
@@ -45,6 +69,10 @@ class Layer {
   virtual void Backward_gpu(const vector<Blob<Dtype>*>& top, const vector<bool>& propagate_down,
                             const vector<Blob<Dtype>*>& bottom) {
     Backward_cpu(top, propagate_down, bottom);
+  }
+  void SetLossWeights(const vector<Blob<Dtype>*>& top) {
+    for (int i = 0; i < layer_param_.loss_weight_size() && i < static_cast<int>(top.size()); ++i)
+      caffe_set(top[i]->count(), Dtype(layer_param_.loss_weight(i)), top[i]->mutable_cpu_diff());
   }
 };
 }  // namespace caffe

@@ -4,7 +4,7 @@ accuracy_seg and their _ext copies), forward and backward, as the median of CUDA
 the training shapes: a 38x63 feature map with A = 9 anchors, stage 1 at the ProposalTargetLayer
 capacity of 64 + 3 rows with a device row count of 64, stage 2 at 67 rows (a StageBridge count of
 64 RoIs + 3 gt boxes).  Targets are synthetic with the target layers' value sets.  When
-oracle/_ref/libmnc_ref_loss.so is built (oracle/loss.mk), the same 14 layers are timed through the
+oracle/_ref/libmnc_ref_loss.so is built (oracle/Makefile), the same 14 layers are timed through the
 reference's own Forward + Backward (CUDA events; its device->host round trips and host loops
 included; Accuracy, CPU-only there, by the host clock).  Prints one JSON line with the card's name
 and power limit.

@@ -6,7 +6,7 @@ events (warm-up, then --iters launches each; the median is reported) at two shap
   infer  the inference batch: 8 images, conv5_3 8x512x38x63, 2400 RoIs (300 per image)
 
 ROIPooling runs at 7x7 (the CFM net's pooled size) on the same RoIs.  When
-oracle/_ref/libmnc_ref_backward.so exists (oracle/backward.mk), the reference's own Backward_gpu is timed on the same
+oracle/_ref/libmnc_ref_backward.so exists (oracle/Makefile), the reference's own Backward_gpu is timed on the same
 inputs through the driver's timed entry points (Backward between events on one set-up layer).
 Our calls are timed as CUDA-graph replays; the reference's as events around its Backward call.
 Prints one JSON line with the card's name and power limit.

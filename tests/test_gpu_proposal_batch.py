@@ -263,7 +263,7 @@ def test_rpn_decode_softmax_is_the_reference_softmax(H, W, cpad):
     image (both builds of the reference library)."""
     libs = [p for p in REF_LOSS_LIBS if os.path.exists(p)]
     if not libs:
-        pytest.skip("reference loss library not built (oracle/loss.mk needs a reference checkout)")
+        pytest.skip("reference loss library not built (oracle/Makefile needs a reference checkout)")
     B = 3
     fg, logits, deltas, kind = decode_case(B, H, W, seed=7 + H * W + cpad)
     logits[0, :, 0, 0] = 0.0                       # bg == fg: exactly 0.5

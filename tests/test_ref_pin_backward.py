@@ -1,5 +1,5 @@
 """Pin the backward passes three ways: the reference's own Backward_gpu (caffe-mnc layer sources
-compiled unmodified into oracle/_ref/libmnc_ref_backward*.so by oracle/backward.mk, driven by
+compiled unmodified into oracle/_ref/libmnc_ref_backward*.so by oracle/Makefile, driven by
 oracle/ref_backward_driver.cu)
 == oracle == CUDA path.  Against the -fmad=false build every feature and mask gradient is
 bit-exact; against the default build they agree to the FMA-rounding tolerance of the forward pins.

@@ -1,5 +1,5 @@
 """Pin of the convolution against the reference's own ConvolutionLayer (conv_layer, base_conv_layer
-and im2col compiled unmodified into oracle/_ref/libmnc_ref_conv*.so by oracle/conv.mk, run as Caffe
+and im2col compiled unmodified into oracle/_ref/libmnc_ref_conv*.so by oracle/Makefile, run as Caffe
 runs it in GPU mode: im2col + sgemm per image, the bias by a gemm / gemv with beta 1).  At the 16
 layer shapes of the training net, for a reduced 150x250 image, and at tail shapes with two images,
 the reference and ours are each held to float64 of the same operands, and ours to the reference
@@ -22,7 +22,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIBS = [os.path.join(ROOT, "oracle", "_ref", n) for n in
         ("libmnc_ref_conv_nofma.so", "libmnc_ref_conv.so")]
 if not all(os.path.exists(p) for p in LIBS):
-    pytest.skip("reference convolution library not built (oracle/conv.mk needs a reference checkout)",
+    pytest.skip("reference convolution library not built (oracle/Makefile needs a reference checkout)",
                 allow_module_level=True)
 F32 = np.float32
 IMAGE = (150, 250)

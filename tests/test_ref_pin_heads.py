@@ -1,5 +1,5 @@
 """Pin of the head layers against the reference's own InnerProduct, Pooling, ReLU and Sigmoid
-(compiled unmodified into oracle/_ref/libmnc_ref_heads*.so by oracle/heads.mk, run as Caffe runs
+(compiled unmodified into oracle/_ref/libmnc_ref_heads*.so by oracle/Makefile, run as Caffe runs
 them in GPU mode).  Pooling, ReLU and Sigmoid, forward and backward, equal both reference builds bit
 for bit.  The reference's InnerProduct (cuBLAS sgemm / sgemv) and ours are each held to float64 of
 the same operands; ours must meet the split-bf16 bound of tests/fc_bound.py, and both max ratios
@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIBS = [os.path.join(ROOT, "oracle", "_ref", n) for n in
         ("libmnc_ref_heads_nofma.so", "libmnc_ref_heads.so")]
 if not all(os.path.exists(p) for p in LIBS):
-    pytest.skip("reference head-layer library not built (oracle/heads.mk needs a reference checkout)",
+    pytest.skip("reference head-layer library not built (oracle/Makefile needs a reference checkout)",
                 allow_module_level=True)
 F32 = np.float32
 

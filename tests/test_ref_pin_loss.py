@@ -1,6 +1,6 @@
 """Three-way pin of the loss layers: the reference's own SoftmaxWithLoss, SmoothL1Loss,
 SigmoidCrossEntropyLoss and Accuracy (compiled unmodified into oracle/_ref/libmnc_ref_loss*.so by
-oracle/loss.mk, run as Caffe runs them in GPU mode) == the numpy oracle == the device, at the
+oracle/Makefile, run as Caffe runs them in GPU mode) == the numpy oracle == the device, at the
 training-net shapes with the targets of the device's own target layers.  Diffs and prob are held
 bit for bit against both builds (the kernels involved contract nothing: no multiply feeds an add),
 accuracy exactly, loss scalars to the error bound of the reference's unordered float sum
@@ -19,7 +19,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIBS = [os.path.join(ROOT, "oracle", "_ref", n) for n in
         ("libmnc_ref_loss_nofma.so", "libmnc_ref_loss.so")]
 if not all(os.path.exists(p) for p in LIBS):
-    pytest.skip("reference loss library not built (oracle/loss.mk needs a reference checkout)",
+    pytest.skip("reference loss library not built (oracle/Makefile needs a reference checkout)",
                 allow_module_level=True)
 F32 = np.float32
 
